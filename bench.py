@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py — ControlLoRA training throughput on B200 (the BASELINE.json metric).
+"""bench.py — ControlLoRA training throughput on one or more H100s (the BASELINE.json metric).
 
   python bench.py --gpus N --steps K --warmup W            # this framework (one process per GPU; torchrun for N > 1)
   python bench.py --impl reference --gpus N --steps K ...   # the reference algorithm's CPU path (oracle port) on host cores
+  python bench.py --gpus 1 --steps K --dump-outputs DIR     # also write the last timed step's results as DIR/<name>.npy
 
 One "step" = hint-encoder fwd + SD-1.5 UNet fwd + MSE + backward (dX, LoRA dA/dB, hint-encoder dW) + gradient
 all-reduce (N > 1) + clip_grad_norm + AdamW, on synthetic 512x512 inputs (64x64 latents, 77x768 text states), batch 8
@@ -30,18 +31,6 @@ UNIT = "images/s"
 GFLOP_PER_IMAGE_STEP = 1794.0
 
 
-def gemm_traffic_per_launch():
-    """DRAM bytes per gemm_tc_kernel launch (dram__bytes_read.sum + dram__bytes_write.sum averaged over the GEMM launches of
-    one training step) from the committed ncu capture profiles/r01_gemm_traffic.json; None when the file is missing."""
-    try:
-        root = Path(__file__).resolve().parent / "profiles"
-        f = root / "r02_gemm_traffic.json"
-        d = json.loads((f if f.exists() else root / "r01_gemm_traffic.json").read_text())
-        return float(d["bytes_per_launch"])
-    except Exception:
-        return None
-
-
 def parse():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -56,6 +45,9 @@ def parse():
     ap.add_argument("--no-aux", action="store_true", help="skip the auxiliary numbers (denoise C3/C5, drop-in path, per-shape GEMM table)")
     ap.add_argument("--aux-only", default=None, choices=["train_from_pixels"],
                     help="run ONE auxiliary measurement in this process and print its JSON (bench.py runs it as an isolated child process)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed (loss, updated trainable parameters) "
+                         "as DIR/<name>.npy; inputs and weights are seeded, so two builds can be compared output for output")
     return ap.parse_args()
 
 
@@ -72,7 +64,7 @@ def synth_inputs(torch, B, seed_off=0, device="cpu"):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe), polled from a thread."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region, polled from a thread."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -123,8 +115,8 @@ def measured_peaks():
     p = ROOT / "MEASURED_PEAKS.json"
     if p.exists():
         d = json.loads(p.read_text())
-        return d.get("bf16_tflops_sustained", 1400.0), d.get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json, sustained bf16)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md: 1.4 PF sustained)"
+        return d.get("bf16_tflops_sustained", 989.0), d.get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json, sustained bf16)"
+    return 989.0, 3350.0, "H100 SXM data sheet (dense bf16, HBM3 at 700 W); not a measured rate"
 
 
 # ------------------------------------------------------------------------------------------------------ CPU oracle arm
@@ -395,10 +387,11 @@ def run_aux_only(a):
 
 
 def aux_gemm_table(torch, ops):
-    """Per-shape throughput of the tcgen05 GEMM family at the SD-1.5 shapes (SURVEY 8a census), each timed ALONE with CUDA
+    """Per-shape throughput of the wgmma GEMM family at the SD-1.5 shapes (SURVEY 8a census), each timed ALONE with CUDA
     events over operand sets that rotate through > 126 MB (so L2 does not hold them), against the burst bf16 peak of
-    MEASURED_PEAKS.json; cuBLAS (torch.matmul) on the same shape is printed beside it for context only."""
-    peak = 1667.1
+    MEASURED_PEAKS.json (else the H100 SXM data sheet's dense bf16 rate); cuBLAS (torch.matmul) on the same shape is printed
+    beside it for context only."""
+    peak = 989.0
     pth = ROOT / "MEASURED_PEAKS.json"
     if pth.exists():
         peak = json.loads(pth.read_text()).get("bf16_tflops", peak)
@@ -455,10 +448,21 @@ def aux_gemm_table(torch, ops):
                      "cublas_us_no_lora": None, "vs_cublas": None})
         del Xs, Ds
     return {"rows": rows, "peak_tflops_burst": peak,
-            "what": "each shape timed alone (CUDA events, operands rotated through >126 MB); frac = TFLOP/s / measured burst bf16 peak"}
+            "what": "each shape timed alone (CUDA events, operands rotated through >126 MB); frac = TFLOP/s / bf16 peak (MEASURED_PEAKS.json burst rate, else the data sheet)"}
 
 
 # ------------------------------------------------------------------------------------------------------ GPU arm
+def dump_outputs(out_dir, loss, flat_p):
+    """What a caller of Trainer.step holds after the last timed step: the loss and the updated trainable parameters (the flat
+    fp32 arena, 5-6 M values = 20-24 MB)."""
+    import numpy as np
+
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    np.save(d / "loss.npy", loss.detach().double().reshape(1).cpu().numpy())
+    np.save(d / "trainable_params.npy", flat_p.detach().float().cpu().numpy())
+
+
 def run_ours(a):
     import torch
     import torch.distributed as dist
@@ -476,6 +480,7 @@ def run_ours(a):
 
     dev = torch.device("cuda", local)
     B = a.batch
+    torch.manual_seed(0)        # the adapters' initialisation: identical weights from run to run
     unet = cb.UNet2DConditionModel.synthetic(dev, seed=0)
     cl = cb.ControlLoRA.from_config(NAMED[a.config]).to(dev)
     g = torch.Generator().manual_seed(3)
@@ -516,6 +521,8 @@ def run_ours(a):
     e1.record()
     barrier()
     ms_total = e0.elapsed_time(e1)
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, loss, tr.flat_p)
     launches = (_lib.launch_count() - n0) // max(a.steps, 1)
     if tr.cuda_graph and tr.launches_per_step:
         launches = tr.launches_per_step      # kernels inside the replayed graph (counted at capture) + optimizer launches
@@ -582,7 +589,7 @@ def run_ours(a):
         dist.all_reduce(dt, op=dist.ReduceOp.MAX)
     e2e_value = world * B * a.steps / float(dt)
 
-    # ---------------- roofline of the dominant kernel family (tcgen05 GEMM / implicit-GEMM conv): live CUDA-event timing
+    # ---------------- roofline of the dominant kernel family (wgmma GEMM / implicit-GEMM conv): live CUDA-event timing
     trace("roofline passes")
     roof = None
     if world > 1 and not a.no_roofline:
@@ -622,8 +629,8 @@ def run_ours(a):
         alg_bytes = sum(r[3] for r in rec)
         ach = fl / (tm * 1e-3) / 1e12
     if rank == 0 and not a.no_roofline:
-        roof = {"bound": "tensor", "kernel": "gemm_tc_kernel<BN,EXT,BK> (all fused linear / LoRA / implicit-GEMM conv launches of one step)",
-                "achieved": ach, "peak": peak_tf, "unit": "TFLOP/s", "frac": ach / peak_tf, "traffic": gemm_traffic_per_launch(),
+        roof = {"bound": "tensor", "kernel": "gemm_wgmma_kernel<BN,EXT,BK> (all fused linear / LoRA / implicit-GEMM conv launches of one step)",
+                "achieved": ach, "peak": peak_tf, "unit": "TFLOP/s", "frac": ach / peak_tf,
                 "launches_per_step": len(rec), "gemm_ms_per_step": tm, "algorithmic_gflop_per_step": fl / 1e9,
                 "algorithmic_bytes_per_step": alg_bytes, "algorithmic_bytes_per_launch": alg_bytes / max(len(rec), 1),
                 "peak_source": which,
@@ -664,7 +671,7 @@ def run_ours(a):
                                    f"batch {B}/GPU, hint encoder + UNet fwd/bwd + clip + AdamW" + (" + NCCL all-reduce of the flat grad arena" if world > 1 else ""),
                        "global_batch": world * B, "parallelism": f"dp{world}", "replicas_in_sync": replicas_in_sync,
                        "cuda_graph": graph_used,
-                       "l2_policy": "no explicit flush: each step streams 1.7 GB of frozen weights plus >5 GB of activations, far beyond the 126 MB L2",
+                       "l2_policy": "no explicit flush: each step streams 1.7 GB of frozen weights plus >5 GB of activations, far beyond the 50 MB L2",
                        "weights": "random-init (seeded), SD-1.5 / ControlLoRA shapes", "final_loss": final_loss},
             "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4},
             "gpu_launches": int(launches),

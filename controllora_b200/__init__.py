@@ -1,4 +1,4 @@
-"""controllora_b200 — B200-native (sm_100a) implementation of the ControlLoRA UNet hot path.
+"""controllora_b200 — H100-native (sm_90a) implementation of the ControlLoRA UNet hot path.
 
 Public surface mirrors /root/reference/models.py plus the slice of diffusers' UNet2DConditionModel that the reference
 drivers use.  Importing the package does not require a GPU; running any op does (there is no CPU fallback).

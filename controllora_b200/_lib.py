@@ -11,8 +11,8 @@ from pathlib import Path
 import os
 
 _PKG = Path(__file__).resolve().parent
-# CLB_LIB selects an instrumented build of the same sources (e.g. the CLB_TIMELINE debug library that
-# `python -m controllora_b200.build --timeline` writes next to the product library); never a different implementation.
+# CLB_LIB selects another build of the same sources (e.g. one compiled with extra CLB_EXTRA_NVCC flags); never a different
+# implementation.
 LIB_PATH = Path(os.environ["CLB_LIB"]) if os.environ.get("CLB_LIB") else _PKG / "libcontrollora_b200.so"
 
 
@@ -44,7 +44,7 @@ def require_cuda(device, what: str) -> None:
     test doubles and only the Python program above the C ABI is being exercised."""
     dev_type = device if isinstance(device, str) else getattr(device, "type", str(device))
     if dev_type != "cuda" and not os.environ.get("CLB_DRYRUN"):
-        raise RuntimeError(f"controllora_b200.{what} runs only on CUDA (sm_100a); there is no CPU path")
+        raise RuntimeError(f"controllora_b200.{what} runs only on CUDA (sm_90a); there is no CPU path")
 
 
 def check(status: int, what: str = "") -> None:

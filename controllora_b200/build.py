@@ -1,6 +1,6 @@
-"""In-tree build of the sm_100a shared library (C ABI declared in include/controllora_b200.h).
+"""In-tree build of the sm_90a (H100) shared library (C ABI declared in include/controllora_b200.h).
 
-`python -m controllora_b200.build` compiles every csrc/*.cu with nvcc for sm_100a and links
+`python -m controllora_b200.build` compiles every csrc/*.cu with nvcc for sm_90a and links
 `controllora_b200/libcontrollora_b200.so`.  Objects are rebuilt only when a source or header is newer.
 """
 from __future__ import annotations
@@ -18,7 +18,7 @@ LIB = PKG / "libcontrollora_b200.so"
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -30,12 +30,7 @@ def _newer(a: Path, b: Path) -> bool:
     return (not b.exists()) or a.stat().st_mtime > b.stat().st_mtime
 
 
-def build(verbose: bool = False, force: bool = False, timeline: bool = False) -> Path:
-    """timeline=True: debug variant with the in-kernel clock64 event log (-DCLB_TIMELINE) -> libcontrollora_b200_tl.so,
-    objects under build_tl/ (select it with CLB_LIB=...; tools/gemm_timeline.py)."""
-    global OBJ, LIB, FLAGS
-    if timeline:
-        OBJ, LIB, FLAGS = PKG / "build_tl", PKG / "libcontrollora_b200_tl.so", FLAGS + ["-DCLB_TIMELINE"]
+def build(verbose: bool = False, force: bool = False) -> Path:
     OBJ.mkdir(exist_ok=True)
     sources = sorted(CSRC.glob("*.cu"))
     headers = list(CSRC.glob("*.cuh")) + list(CSRC.glob("*.h")) + list((PKG.parent / "include").glob("*.h"))
@@ -70,5 +65,5 @@ def build(verbose: bool = False, force: bool = False, timeline: bool = False) ->
 
 
 if __name__ == "__main__":
-    p = build(verbose="-v" in sys.argv, force="-f" in sys.argv, timeline="--timeline" in sys.argv)
+    p = build(verbose="-v" in sys.argv, force="-f" in sys.argv)
     print(p)

@@ -1,4 +1,4 @@
-"""`CLIPTextModel` — the frozen text encoder in front of the hot path (SURVEY.md 8f rank 3), on the same sm_100a kernels:
+"""`CLIPTextModel` — the frozen text encoder in front of the hot path (SURVEY.md 8f rank 3), on the same sm_90a kernels:
 
   encoder_hidden_states = text_encoder(batch["input_ids"])[0]                  train_text_to_image_control_lora.py:768
   (and the prompt embeddings of the pipelines, train_…:829-843, apps/gradio_*2image.py, mix_lora_and_control_lora.py)

@@ -1,0 +1,312 @@
+// K2 (backward) — flash-attention backward for sm_90a on wgmma, what torch autograd derives for the reference's baddbmm /
+// softmax / bmm (models.py:140-141, 270-271, 407-408).  P is recomputed from Q, K and the forward's log2-domain LSE;
+// delta = rowsum(dO * O) comes from a small kernel first.  Both kernels use three warpgroups: a TMA producer (one elected
+// thread: the CTA's own tiles once, then a two-stage mbarrier ring of the streamed tiles) and two consumer warpgroups of 64
+// rows each, whose products run on wgmma with the accumulators in registers and P / dS fed back as register A operands.
+//
+//   dKV kernel: one CTA = 128 keys of one (batch, head); it streams Q / dO tiles of 64 queries (32 for heads wider than 64):
+//               S^T = K Q^T -> P^T,  dV += P^T dO,  dP^T = V dO^T,  dS^T = P^T (dP^T - delta),  dK += dS^T Q
+//               (heads wider than 128 split the dK / dV columns over two CTAs to bound the accumulator registers)
+//   dQ kernel:  one CTA = 128 queries; it streams K / V tiles of 64 keys (32 for heads wider than 64):
+//               S = Q K^T -> P,  dP = dO V^T,  dS = P (dP - delta),  dQ += dS K
+// No atomics: every output element is written by exactly one thread.
+#include <stdio.h>
+#include <stdlib.h>
+#include <string.h>
+
+#include "common.cuh"
+#include "attention_tile.cuh"
+#define CLB_FAMILY 2      // CLB_PDL_MASK bit of this file's kernels
+#include "host_common.h"
+#include "../../include/controllora_b200.h"
+
+namespace clb {
+
+struct AttnBwdParams {
+    int B, H, Nq, Nk, d;
+    const float* lse;
+    const float* delta;
+    __nv_bfloat16* dq; long long lddq;
+    __nv_bfloat16* dk; long long lddk;
+    __nv_bfloat16* dv; long long lddv;
+    float scale, scale_log2;
+    int num_blocks;
+};
+
+template <int DCH>
+struct BwdCfg {
+    static constexpr int BI = (DCH == 1) ? 64 : 32;        // streamed rows per stage (queries for dKV, keys for dQ): register budget
+    static constexpr int OUTC = DCH < 2 ? DCH : 2;         // dK / dV column chunks per dKV CTA
+    static constexpr int FIX_BYTES = DCH * 128 * 128;      // one of the CTA's own 128-row tiles
+    static constexpr int IN_BYTES = DCH * BI * 128;        // one streamed tile
+    static constexpr int STAGE_BYTES = 2 * IN_BYTES;
+    static constexpr int STAGES = 2;
+    static constexpr int SMEM_BYTES = 1024 + 2 * FIX_BYTES + STAGES * STAGE_BYTES + 256;
+};
+
+// the shared producer: fixed tiles f0 / f1 (128 rows from frow0) once, then n tiles of BI rows of s0 / s1 through the ring
+template <int DCH>
+__device__ __forceinline__ void bwd_produce(const CUtensorMap* f0, const CUtensorMap* f1, int frow0, const CUtensorMap* s0,
+                                            const CUtensorMap* s1, int n, uint8_t* sfix, uint8_t* sin, uint64_t* fix_bar,
+                                            uint64_t* full_bar, uint64_t* empty_bar, int h, int b) {
+    using Cfg = BwdCfg<DCH>;
+    mbar_arrive_expect_tx(fix_bar, 2 * Cfg::FIX_BYTES);
+    load_head_tile<DCH, 128>(f0, fix_bar, sfix, h, frow0, b);
+    load_head_tile<DCH, 128>(f1, fix_bar, sfix + Cfg::FIX_BYTES, h, frow0, b);
+    int stage = 0; uint32_t phase = 0;
+    for (int j = 0; j < n; ++j) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
+        uint8_t* st = sin + stage * Cfg::STAGE_BYTES;
+        load_head_tile<DCH, Cfg::BI>(s0, &full_bar[stage], st, h, j * Cfg::BI, b);
+        load_head_tile<DCH, Cfg::BI>(s1, &full_bar[stage], st + Cfg::IN_BYTES, h, j * Cfg::BI, b);
+        if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+    }
+}
+
+#define BWD_PROLOGUE                                                                                                     \
+    extern __shared__ __align__(1024) uint8_t smem_raw[];                                                                \
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));      \
+    uint8_t* sfix = smem;                                                                                                \
+    uint8_t* sin = sfix + 2 * Cfg::FIX_BYTES;                                                                            \
+    uint64_t* fix_bar = reinterpret_cast<uint64_t*>(sin + Cfg::STAGES * Cfg::STAGE_BYTES);                               \
+    uint64_t* full_bar = fix_bar + 1;                                                                                    \
+    uint64_t* empty_bar = full_bar + Cfg::STAGES;                                                                        \
+    const int warp_idx = uniform_warp_idx(), lane = threadIdx.x & 31;                                                    \
+    const int wg = warp_idx >> 2;                                                                                        \
+    if (threadIdx.x == 0) {                                                                                              \
+        mbar_init(fix_bar, 1);                                                                                           \
+        for (int i = 0; i < Cfg::STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 2); }              \
+        fence_barrier_init();                                                                                            \
+    }                                                                                                                    \
+    __syncthreads();                                                                                                     \
+    pdl_wait();
+
+template <int DCH>
+__global__ void __launch_bounds__(ATT_THREADS, 1)
+attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                    const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO, const AttnBwdParams p) {
+    pdl_launch_dependents();
+    using Cfg = BwdCfg<DCH>;
+    constexpr int BI = Cfg::BI, OUTC = Cfg::OUTC;
+    BWD_PROLOGUE
+    int bid = blockIdx.x;
+    const int kb = bid % p.num_blocks; bid /= p.num_blocks;
+    const int h = bid % p.H, b = bid / p.H;
+    const int k0 = kb * 128, c0 = blockIdx.y * OUTC;
+    const int nqb = (p.Nq + BI - 1) / BI;
+    if (wg == 0) {
+        setmaxnreg_dec<40>();
+        if (warp_idx == 0 && elect_one_sync())
+            bwd_produce<DCH>(&tmK, &tmV, k0, &tmQ, &tmDO, nqb, sfix, sin, fix_bar, full_bar, empty_bar, h, b);
+        return;
+    }
+    setmaxnreg_inc<232>();
+    const int row0 = (wg - 1) * 64, w4 = warp_idx & 3;
+    const float* glse = p.lse + ((long long)b * p.H + h) * p.Nq;
+    const float* gdelta = p.delta + ((long long)b * p.H + h) * p.Nq;
+    float dk[OUTC][32], dv[OUTC][32];
+#pragma unroll
+    for (int c = 0; c < OUTC; ++c)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) dk[c][i] = dv[c][i] = 0.f;
+    mbar_wait(fix_bar, 0);
+    const uint32_t k_addr = smem_u32(sfix), v_addr = k_addr + Cfg::FIX_BYTES;
+    int stage = 0; uint32_t phase = 0;
+    for (int j = 0; j < nqb; ++j) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t q_addr = smem_u32(sin + stage * Cfg::STAGE_BYTES), do_addr = q_addr + Cfg::IN_BYTES;
+        float s[BI / 2];
+        att_abt<DCH, 128, BI>(s, k_addr, row0, q_addr);           // S^T[64 keys][BI queries]
+        float lse_c[BI / 4], dl_c[BI / 4];                          // this lane's query columns 8nt + 2(lane%4) + {0,1}
+#pragma unroll
+        for (int nt = 0; nt < BI / 8; ++nt)
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+                const int qq = j * BI + nt * 8 + 2 * (lane & 3) + c;
+                lse_c[nt * 2 + c] = (qq < p.Nq) ? __ldg(glse + qq) : INFINITY;     // P = 0 for padding queries
+                dl_c[nt * 2 + c] = (qq < p.Nq) ? __ldg(gdelta + qq) : 0.f;
+            }
+#pragma unroll
+        for (int nt = 0; nt < BI / 8; ++nt)
+#pragma unroll
+            for (int c = 0; c < 4; ++c) s[nt * 4 + c] = fast_exp2(s[nt * 4 + c] * p.scale_log2 - lse_c[nt * 2 + (c & 1)]);
+        uint32_t pa[BI / 16][4];
+        acc_to_a<BI / 8>(s, pa);
+        att_pv<OUTC, BI, BI / 16>(dv, pa, do_addr, c0, DCH);    // dV += P^T dO
+        float dp[BI / 2];
+        att_abt<DCH, 128, BI>(dp, v_addr, row0, do_addr);        // dP^T = V dO^T
+#pragma unroll
+        for (int nt = 0; nt < BI / 8; ++nt)
+#pragma unroll
+            for (int c = 0; c < 4; ++c) dp[nt * 4 + c] = s[nt * 4 + c] * (dp[nt * 4 + c] - dl_c[nt * 2 + (c & 1)]);
+        acc_to_a<BI / 8>(dp, pa);
+        att_pv<OUTC, BI, BI / 16>(dk, pa, q_addr, c0, DCH);     // dK += dS^T Q
+        if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[stage]);
+        if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+    }
+    store_rows<OUTC>(dk, p.scale, p.dk + (long long)b * p.Nk * p.lddk + h * p.d, p.lddk, k0 + row0, p.Nk, p.d, c0, lane, w4);
+    store_rows<OUTC>(dv, 1.f, p.dv + (long long)b * p.Nk * p.lddv + h * p.d, p.lddv, k0 + row0, p.Nk, p.d, c0, lane, w4);
+}
+
+template <int DCH>
+__global__ void __launch_bounds__(ATT_THREADS, 1)
+attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                   const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO, const AttnBwdParams p) {
+    pdl_launch_dependents();
+    using Cfg = BwdCfg<DCH>;
+    constexpr int BI = Cfg::BI;
+    BWD_PROLOGUE
+    int bid = blockIdx.x;
+    const int qb = bid % p.num_blocks; bid /= p.num_blocks;
+    const int h = bid % p.H, b = bid / p.H;
+    const int q0 = qb * 128;
+    const int nkb = (p.Nk + BI - 1) / BI;
+    if (wg == 0) {
+        setmaxnreg_dec<40>();
+        if (warp_idx == 0 && elect_one_sync())
+            bwd_produce<DCH>(&tmQ, &tmDO, q0, &tmK, &tmV, nkb, sfix, sin, fix_bar, full_bar, empty_bar, h, b);
+        return;
+    }
+    setmaxnreg_inc<232>();
+    const int row0 = (wg - 1) * 64, w4 = warp_idx & 3;
+    float lse[2], delta[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        const int qq = q0 + row0 + w4 * 16 + (lane >> 2) + 8 * i;
+        const long long si = ((long long)b * p.H + h) * p.Nq + qq;
+        lse[i] = (qq < p.Nq) ? p.lse[si] : INFINITY;
+        delta[i] = (qq < p.Nq) ? p.delta[si] : 0.f;
+    }
+    float dq[DCH][32];
+#pragma unroll
+    for (int c = 0; c < DCH; ++c)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) dq[c][i] = 0.f;
+    mbar_wait(fix_bar, 0);
+    const uint32_t q_addr = smem_u32(sfix), do_addr = q_addr + Cfg::FIX_BYTES;
+    int stage = 0; uint32_t phase = 0;
+    for (int j = 0; j < nkb; ++j) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t k_addr = smem_u32(sin + stage * Cfg::STAGE_BYTES), v_addr = k_addr + Cfg::IN_BYTES;
+        float s[BI / 2];
+        att_abt<DCH, 128, BI>(s, q_addr, row0, k_addr);           // S[64 queries][BI keys]
+#pragma unroll
+        for (int nt = 0; nt < BI / 8; ++nt)
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+                const int key = j * BI + nt * 8 + 2 * (lane & 3) + (c & 1);
+                s[nt * 4 + c] = (key < p.Nk) ? fast_exp2(s[nt * 4 + c] * p.scale_log2 - lse[c >> 1]) : 0.f;
+            }
+        float dp[BI / 2];
+        att_abt<DCH, 128, BI>(dp, do_addr, row0, v_addr);        // dP = dO V^T
+#pragma unroll
+        for (int nt = 0; nt < BI / 8; ++nt)
+#pragma unroll
+            for (int c = 0; c < 4; ++c) dp[nt * 4 + c] = s[nt * 4 + c] * (dp[nt * 4 + c] - delta[c >> 1]);
+        uint32_t pa[BI / 16][4];
+        acc_to_a<BI / 8>(dp, pa);
+        att_pv<DCH, BI, BI / 16>(dq, pa, k_addr, 0, DCH);        // dQ += dS K
+        if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[stage]);
+        if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+    }
+    store_rows<DCH>(dq, p.scale, p.dq + (long long)b * p.Nq * p.lddq + h * p.d, p.lddq, q0 + row0, p.Nq, p.d, 0, lane, w4);
+}
+
+// ===================================================================================================== delta
+// delta[b, h, q] = sum_d dO[b, q, h*d + :] * O[b, q, h*d + :]
+__global__ void attn_delta_kernel(const __nv_bfloat16* __restrict__ o, long long ldo, const __nv_bfloat16* __restrict__ d_o,
+                                  long long lddo, float* __restrict__ delta, int B, int H, int Nq, int d) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const long long total = (long long)B * Nq * H;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const int h = (int)(i % H);
+        const long long bq = i / H;
+        const int q = (int)(bq % Nq);
+        const int b = (int)(bq / Nq);
+        const __nv_bfloat16* po = o + bq * ldo + h * d;
+        const __nv_bfloat16* pd = d_o + bq * lddo + h * d;
+        float s = 0.f;
+        for (int c = 0; c < d; c += 8) {
+            const uint4 a = *reinterpret_cast<const uint4*>(po + c);
+            const uint4 g = *reinterpret_cast<const uint4*>(pd + c);
+            const float2 a0 = unpack_bf16x2(a.x), a1 = unpack_bf16x2(a.y), a2 = unpack_bf16x2(a.z), a3 = unpack_bf16x2(a.w);
+            const float2 g0 = unpack_bf16x2(g.x), g1 = unpack_bf16x2(g.y), g2 = unpack_bf16x2(g.z), g3 = unpack_bf16x2(g.w);
+            s += a0.x * g0.x + a0.y * g0.y + a1.x * g1.x + a1.y * g1.y + a2.x * g2.x + a2.y * g2.y + a3.x * g3.x + a3.y * g3.y;
+        }
+        delta[((long long)b * H + h) * Nq + q] = s;
+    }
+}
+
+template <int DCH>
+static int launch_attn_bwd(const cl_attn_bwd_args* a, cudaStream_t stream) {
+    using Cfg = BwdCfg<DCH>;
+    AttnBwdParams p;
+    p.B = a->B; p.H = a->H; p.Nq = a->Nq; p.Nk = a->Nk; p.d = a->d;
+    p.lse = a->lse; p.delta = a->delta;
+    p.dq = reinterpret_cast<__nv_bfloat16*>(a->dq); p.lddq = a->lddq;
+    p.dk = reinterpret_cast<__nv_bfloat16*>(a->dk); p.lddk = a->lddk;
+    p.dv = reinterpret_cast<__nv_bfloat16*>(a->dv); p.lddv = a->lddv;
+    p.scale = a->scale; p.scale_log2 = a->scale * 1.4426950408889634f;
+    {
+        const long long total = (long long)a->B * a->Nq * a->H;
+        int blocks = (int)((total + 255) / 256);
+        if (blocks > num_sms() * 8) blocks = num_sms() * 8;
+        launch_k(attn_delta_kernel, blocks, 256, 0, stream, reinterpret_cast<const __nv_bfloat16*>(a->o), a->ldo,
+                                                      reinterpret_cast<const __nv_bfloat16*>(a->d_o), a->lddo, a->delta,
+                                                      a->B, a->H, a->Nq, a->d);
+        count_launch();
+    }
+    static bool attr_done = false;
+    if (!attr_done) {
+        CL_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_dkv_kernel<DCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+        CL_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_dq_kernel<DCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+        attr_done = true;
+    }
+    if (a->dk != nullptr) {
+        CUtensorMap tq, tk, tv, tdo;
+        CL_CHECK(make_head_map(&tq, a->q, a->B, a->H, a->Nq, a->d, a->ldq, Cfg::BI));
+        CL_CHECK(make_head_map(&tdo, a->d_o, a->B, a->H, a->Nq, a->d, a->lddo, Cfg::BI));
+        CL_CHECK(make_head_map(&tk, a->k, a->B, a->H, a->Nk, a->d, a->ldk, 128));
+        CL_CHECK(make_head_map(&tv, a->v, a->B, a->H, a->Nk, a->d, a->ldv, 128));
+        p.num_blocks = (a->Nk + 127) / 128;
+        const long long grid = (long long)a->B * a->H * p.num_blocks;
+        if (grid > 0x7fffffffLL) return set_error(CL_ERR_UNSUPPORTED, "cl_attn_bwd: too many blocks");
+        launch_k(attn_bwd_dkv_kernel<DCH>, dim3((unsigned)grid, (DCH + Cfg::OUTC - 1) / Cfg::OUTC), ATT_THREADS, Cfg::SMEM_BYTES,
+                 stream, tq, tk, tv, tdo, p);
+        count_launch();
+    }
+    if (a->dq != nullptr) {
+        CUtensorMap tq, tk, tv, tdo;
+        CL_CHECK(make_head_map(&tq, a->q, a->B, a->H, a->Nq, a->d, a->ldq, 128));
+        CL_CHECK(make_head_map(&tdo, a->d_o, a->B, a->H, a->Nq, a->d, a->lddo, 128));
+        CL_CHECK(make_head_map(&tk, a->k, a->B, a->H, a->Nk, a->d, a->ldk, Cfg::BI));
+        CL_CHECK(make_head_map(&tv, a->v, a->B, a->H, a->Nk, a->d, a->ldv, Cfg::BI));
+        p.num_blocks = (a->Nq + 127) / 128;
+        const long long grid = (long long)a->B * a->H * p.num_blocks;
+        if (grid > 0x7fffffffLL) return set_error(CL_ERR_UNSUPPORTED, "cl_attn_bwd: too many blocks");
+        launch_k(attn_bwd_dq_kernel<DCH>, (unsigned)grid, ATT_THREADS, Cfg::SMEM_BYTES, stream, tq, tk, tv, tdo, p);
+        count_launch();
+    }
+    CL_CUDA_CHECK(cudaGetLastError());
+    return CL_OK;
+}
+
+}  // namespace clb
+
+using namespace clb;
+
+extern "C" int cl_attn_bwd(const cl_attn_bwd_args* a, void* stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    if (!a || !a->q || !a->k || !a->v || !a->o || !a->d_o || !a->lse || !a->delta)
+        return set_error(CL_ERR_INVALID, "cl_attn_bwd: null pointer");
+    if ((a->dk == nullptr) != (a->dv == nullptr)) return set_error(CL_ERR_INVALID, "cl_attn_bwd: dk and dv go together");
+    if (a->d % 8 != 0 || a->d <= 0 || a->d > 192) return set_error(CL_ERR_UNSUPPORTED, "cl_attn_bwd: head dim must be a multiple of 8, <= 192");
+    if ((a->ldq % 8) || (a->ldk % 8) || (a->ldv % 8) || (a->ldo % 8) || (a->lddo % 8) || (a->dq && a->lddq % 8) ||
+        (a->dk && ((a->lddk % 8) || (a->lddv % 8))))
+        return set_error(CL_ERR_INVALID, "cl_attn_bwd: row strides must be multiples of 8");
+    if (a->d <= 64) return launch_attn_bwd<1>(a, stream);
+    if (a->d <= 128) return launch_attn_bwd<2>(a, stream);
+    return launch_attn_bwd<3>(a, stream);
+}

@@ -1,4 +1,4 @@
-// Shared device helpers for the sm_100a kernels: mbarrier / TMA / tcgen05 PTX wrappers.
+// Shared device helpers for the sm_90a kernels: mbarrier / TMA / wgmma / mma.sync PTX wrappers.
 // Everything here is hand-written inline PTX (no CUTLASS/CuTe in the product path).
 #pragma once
 #include <cuda_runtime.h>
@@ -63,17 +63,15 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
         : "memory");
     return ok != 0;
 }
-// Bounded spin: a protocol bug must surface as a trap (-> CUDA error), never as a hung GPU box.
+// Bounded spin: a protocol bug must surface as a trap (-> CUDA error), never as a hung GPU.  (No printf here: a call inside
+// the consumer loops makes ptxas serialise every wgmma of the kernel.)
 #ifndef CLB_MBAR_SPIN_LIMIT
 #define CLB_MBAR_SPIN_LIMIT (1u << 22)
 #endif
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     uint32_t spins = 0;
     while (!mbar_try_wait(bar, parity)) {
-        if (++spins > CLB_MBAR_SPIN_LIMIT) {
-            printf("clb: mbarrier wait timeout (block %d,%d thread %d)\n", blockIdx.x, blockIdx.y, threadIdx.x);
-            __trap();
-        }
+        if (++spins > CLB_MBAR_SPIN_LIMIT) __trap();
     }
 }
 
@@ -131,7 +129,7 @@ template <int N> __device__ __forceinline__ void bulk_wait_group_read() {
     asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
 }
 
-// ---------------------------------------------------------------- CTA pairs (thread-block cluster of 2, cta_group::2)
+// ---------------------------------------------------------------- thread-block clusters
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -146,206 +144,40 @@ __device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
     return r;
 }
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA loads of a CTA pair: data lands in THIS CTA's smem, the byte count is credited to the mbarrier at cluster address
-// `mbar_cluster` (the leader CTA's barrier, which the single MMA-issuing thread of the pair waits on).
-__device__ __forceinline__ void tma_load_2d_cg2(const CUtensorMap* m, uint32_t mbar_cluster, void* dst, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(mbar_cluster), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_cg2(const CUtensorMap* m, uint32_t mbar_cluster, void* dst, int c0, int c1,
-                                                int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, "
-        "%6}], [%2];" ::"r"(smem_u32(dst)),
-        "l"(reinterpret_cast<uint64_t>(m)), "r"(mbar_cluster), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_5d_cg2(const CUtensorMap* m, uint32_t mbar_cluster, void* dst, int c0, int c1,
-                                                int c2, int c3, int c4) {
-    asm volatile(
-        "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, "
-        "%6, %7}], [%2];" ::"r"(smem_u32(dst)),
-        "l"(reinterpret_cast<uint64_t>(m)), "r"(mbar_cluster), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_cg2(uint32_t* smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_cg2() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_cg2(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// commit of the pair's MMAs: arrive on the barrier at this smem offset in every CTA of `cta_mask`
-__device__ __forceinline__ void tc_commit_cg2(uint64_t* bar, uint16_t cta_mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"(cta_mask)
-                 : "memory");
-}
-// D[tmem of both CTAs, 256 x N] (+)= A[128 rows per CTA] * B[N/2 rows per CTA]; issued by the leader CTA only.
-__device__ __forceinline__ void tc_mma_ss_cg2(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                              uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
+
+// ---------------------------------------------------------------- wgmma (sm_90a warpgroup MMA)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator accesses across an in-flight wgmma
+template <int R> __device__ __forceinline__ void wgmma_fence_acc(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-                 "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// tcgen05.commit: arrive on an mbarrier once all previously issued MMAs of this thread retire.
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; bf16 inputs, fp32 accumulate.
-__device__ __forceinline__ void tc_mma_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// A operand from TMEM.
-__device__ __forceinline__ void tc_mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-        "}\n" ::"r"(d_tmem),
-        "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-// Instruction descriptor, kind::f16: bf16 x bf16 -> fp32 (bit layout per the PTX ISA "Instruction descriptor").
-//   [4,6) D format (1 = f32)  [7,10) A format (1 = bf16)  [10,13) B format (1 = bf16)
-//   [15] A major (0 = K)  [16] B major (0 = K)  [17,23) N>>3  [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | (uint32_t(a_mn_major) << 15) | (uint32_t(b_mn_major) << 16) |
-           (uint32_t(N >> 3) << 17) | (uint32_t(M >> 4) << 24);
-}
-
-// Shared-memory matrix descriptor (sm_100 "version 1"):
+// Shared-memory matrix descriptor of wgmma:
 //   [0,14) start address >> 4   [16,30) leading-dim byte offset >> 4   [32,46) stride-dim byte offset >> 4
-//   [46,48) version = 1         [61,64) swizzle: 0 none, 2 = 128B, 4 = 64B, 6 = 32B
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                   uint32_t layout_type, uint32_t base_offset = 0) {
-    uint64_t d = uint64_t(base_offset & 7u) << 49;     // start address not aligned to the swizzle repeat (shifted-row operands)
-    d |= uint64_t((saddr & 0x3FFFFu) >> 4);
+//   [49,52) base offset         [62,64) swizzle: 0 none, 1 = 128B, 2 = 64B, 3 = 32B
+// K-major swizzled operands: rows of 128 (or 64) bytes, 8-row atoms `sbo` bytes apart; a K16 step inside the atom advances
+// the start address by 32 bytes.  MN-major operands: 64 (128B swizzle) MN-contiguous elements per row, one row per k,
+// 8-row k groups `sbo` bytes apart, MN atoms `lbo` bytes apart.
+static constexpr uint32_t SWZ_128B = 1, SWZ_64B = 2;
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t swizzle) {
+    uint64_t d = uint64_t((saddr & 0x3FFFFu) >> 4);
     d |= uint64_t((lbo_bytes >> 4) & 0x3FFFu) << 16;
     d |= uint64_t((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= uint64_t(1) << 46;
-    d |= uint64_t(layout_type & 7u) << 61;
+    d |= uint64_t(swizzle & 3u) << 62;
     return d;
 }
 
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns (thread i = lane i of the warp's quadrant).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-          "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-          "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x16(uint32_t taddr, const uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-        "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-        "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-        : "memory");
-}
-
-// Per-warpgroup register re-budgeting (all 4 warps of the warpgroup execute it): producer warps give registers back,
-// math warps take them.
 // named CTA barriers (id 1..15): arrive = announce and continue, sync = wait for `count` threads
 __device__ __forceinline__ void named_bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 __device__ __forceinline__ void named_bar_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
+// Per-warpgroup register re-budgeting (all 4 warps of the warpgroup execute it): producer warps give registers back,
+// math warps take them.
 template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 
-// registers -> TMEM, same shape as tmem_ld_32x32
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-        "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-        "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]),
-        "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]),
-        "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-        : "memory");
-}
-// registers -> TMEM: this warp's 32 lanes x 8 consecutive 32-bit columns (e.g. 16 packed bf16 values per lane)
-__device__ __forceinline__ void tmem_st_32x8(uint32_t taddr, const uint32_t (&v)[8]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(v[0]), "r"(v[1]),
-        "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
-}
-
-// ---------------------------------------------------------------- warp-converged issue ("_e" = elected)
-// The producer / MMA warps run their loops with all 32 lanes converged and call these: every lane evaluates the (warp-
-// uniform) operands, elect.sync picks one lane - always the same one for the full mask, which tcgen05.commit relies on -
-// and only that lane executes the instruction.  Because nothing depends on the lane id, ptxas keeps addresses, descriptors
-// and coordinates in uniform registers and feeds UTMALDG / UTCHMMA directly, instead of the ELECT + R2UR.BROADCAST
-// "waterfall" it has to emit for a per-thread value under `if (lane == 0)` (~150 clk per tcgen05.mma, round-2 probe).
-__device__ __forceinline__ void mbar_arrive_expect_tx_e(uint64_t* bar, uint32_t bytes) { if (elect_one_sync()) mbar_arrive_expect_tx(bar, bytes); }
-__device__ __forceinline__ void tma_load_2d_e(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1) { if (elect_one_sync()) tma_load_2d(m, bar, dst, c0, c1); }
-__device__ __forceinline__ void tma_load_3d_e(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1, int c2) { if (elect_one_sync()) tma_load_3d(m, bar, dst, c0, c1, c2); }
-__device__ __forceinline__ void tma_load_4d_e(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1, int c2, int c3) { if (elect_one_sync()) tma_load_4d(m, bar, dst, c0, c1, c2, c3); }
-__device__ __forceinline__ void tma_load_5d_e(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1, int c2, int c3, int c4) { if (elect_one_sync()) tma_load_5d(m, bar, dst, c0, c1, c2, c3, c4); }
-__device__ __forceinline__ void bulk_copy_g2s_e(void* dst_smem, const void* src, uint32_t bytes, uint64_t* bar) { if (elect_one_sync()) bulk_copy_g2s(dst_smem, src, bytes, bar); }
-__device__ __forceinline__ void tc_commit_e(uint64_t* bar) { if (elect_one_sync()) tc_commit(bar); }
-__device__ __forceinline__ void tc_mma_ss_e(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) { if (elect_one_sync()) tc_mma_ss(d_tmem, adesc, bdesc, idesc, accumulate); }
-__device__ __forceinline__ void tc_mma_ts_e(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) { if (elect_one_sync()) tc_mma_ts(d_tmem, a_tmem, bdesc, idesc, accumulate); }
 __device__ __forceinline__ int uniform_warp_idx() { return __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0); }
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
@@ -389,22 +221,6 @@ __device__ __forceinline__ float fast_exp2(float x) {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
-}
-
-// 2^x on the FMA / ALU pipes (no MUFU): round-to-nearest split x = n + f through the 1.5 * 2^23 magic add, 2^f on
-// [-0.5, 0.5] as a degree-4 polynomial (relative error < 5e-5, far below the bf16 rounding of P), n added to the exponent.
-// NOT used by the attention kernels: measured on B200 (round 2), alternating it with ex2.approx in the softmax loops made the
-// forward 1.7x SLOWER (494 -> 849 us at 4096^2, d = 40): the ~10 extra FMA / ALU instructions per element cost more issue
-// slots than the MUFU slot they free (the loops are issue-bound: ncu IPC 1.3-1.8 of 4 with XU at 53 %).  Kept for reference.
-__device__ __forceinline__ float exp2_poly(float x) {
-    x = fmaxf(x, -125.0f);
-    const float t = x + 12582912.0f;               // 0x4B400000: low mantissa bits of t = round(x)
-    const float f = x - (t - 12582912.0f);
-    float r = fmaf(f, 0.0096181291f, 0.0555041087f);
-    r = fmaf(r, f, 0.2402265070f);
-    r = fmaf(r, f, 0.6931471806f);
-    r = fmaf(r, f, 1.0f);
-    return __int_as_float(__float_as_int(r) + (__float_as_int(t) << 23));
 }
 
 __device__ __forceinline__ float warp_sum(float v) {

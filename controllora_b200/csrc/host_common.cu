@@ -26,12 +26,9 @@ int set_error(int code, const char* fmt, ...) {
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 
 bool pdl_enabled(int family) {
-    // Programmatic dependent launch, measured on B200 in the CUDA-graph replay of the train step (round 2, per family):
-    //   off 39.39 ms | GEMM only 39.15 | attention only 39.54 | GroupNorm/LayerNorm only 40.66 | LoRA kernels only 39.92 | all 41.19
-    // A dependent grid that starts while its predecessor drains lands on the SMs that free up first; kernels with several CTAs
-    // per SM then pile onto those SMs and run unbalanced, so only the one-CTA-per-SM persistent GEMM (whose prologue - barrier
-    // init, TMEM allocation, descriptor prefetch - is what gets hidden, 2-3 us per launch back to back) carries the attribute
-    // by default.  CLB_PDL=0 disables, CLB_PDL_MASK selects other families (bits: see host_common.h).
+    // Programmatic dependent launch.  A dependent grid that starts while its predecessor drains lands on the SMs that free up
+    // first; kernels with several CTAs per SM then pile onto those SMs and run unbalanced, so only the GEMM (one CTA per SM, whose
+    // prologue - barrier init, descriptor prefetch - is what gets hidden) carries the attribute by default.  CLB_PDL=0 disables, CLB_PDL_MASK selects other families (bits: see host_common.h).
     static const bool on = [] { const char* e = getenv("CLB_PDL"); return !(e && e[0] == '0'); }();
     static const int mask = [] { const char* e = getenv("CLB_PDL_MASK"); return e ? atoi(e) : 1; }();
     return on && (mask & family) != 0;
@@ -43,7 +40,7 @@ int num_sms() {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        if (sms <= 0) sms = 148;
+        if (sms <= 0) sms = 132;
     }
     return sms;
 }

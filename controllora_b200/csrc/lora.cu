@@ -1,6 +1,6 @@
 // LoRA side-path kernels: operand packing for the fused GEMM epilogue and the skinny rank-r reductions of the
 // backward pass (dA, dB) — everything that models.py:89-97,185 (LoRALinearLayer instances) adds to autograd, minus
-// the parts already folded into the tcgen05 GEMM.  All HBM-bound: each activation matrix is read exactly once.
+// the parts already folded into the wgmma GEMM.  All HBM-bound: each activation matrix is read exactly once.
 #include <stdio.h>
 
 #include "common.cuh"

@@ -35,8 +35,8 @@ __device__ __forceinline__ void store8(__nv_bfloat16* p, const float (&f)[8]) {
 //            multiple of C/8) so per-channel partial sums stay in registers; 2 CTAs per SM, 2 rows in flight per thread
 //   coef     one tiny kernel turns the sums into per-(image, channel) affine coefficient arrays
 //   apply    a flat, high-occupancy elementwise pass: one 16-byte chunk per thread-iteration, coefficients read as
-//            float4 from the (L1-resident) arrays - measured on B200, the register-resident-coefficient slab variant of
-//            this pass ran at 35 % of the HBM rate because only one 480-thread CTA fitted per SM.
+//            float4 from the (L1-resident) arrays (a slab variant with register-resident coefficients fits only one 480-thread CTA
+//            per SM).
 // Scratch `ws` (cl_groupnorm_ws_bytes): [n*G*2 fp64 group sums][4 x n*C fp32 coefficients][2 x n*C fp32 channel sums].
 
 static constexpr int GN_MAX_CHUNKS = 512;  // C <= 4096

@@ -1,4 +1,4 @@
-// K6 — weight gradients of the (trainable) hint-encoder convolutions on tcgen05, plus the small helper kernels the
+// K6 — weight gradients of the (trainable) hint-encoder convolutions on wgmma, plus the small helper kernels the
 // hint encoder needs every step (weight re-layout fp32 -> bf16, bias gradient, conv_in weight gradient).
 //
 //   dW[co, ci, ky, kx] += sum_{n,h,w} dY[n, h, w, co] * X[n, s*h + ky - pad, s*w + kx - pad, ci]
@@ -13,6 +13,7 @@
 #include <string.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 #define CLB_FAMILY 64      // CLB_PDL_MASK bit of this file's kernels
 #include "host_common.h"
 #include "../../include/controllora_b200.h"
@@ -31,25 +32,25 @@ struct WgradParams {
     float alpha;
 };
 
-static constexpr int WG_NT = 64;          // input-channel tile (UMMA N)
+static constexpr int WG_NT = 64;          // input-channel tile (wgmma N)
 static constexpr int WG_TG = 3;           // taps per group
 static constexpr int WG_STAGES = 2;
+static constexpr int WG_THREADS = 384;    // producer warpgroup + two consumer warpgroups (64 output channels each)
 static constexpr int WG_A_BYTES = 2 * 128 * 128;              // dY tile: 2 chunks x [128 px x 64 ch]
 static constexpr int WG_B_BYTES = 128 * 128;                  // one X tile: [128 px x 64 ch]
 static constexpr int WG_STAGE_BYTES = WG_A_BYTES + WG_TG * WG_B_BYTES;
 static constexpr int WG_SMEM = 1024 + WG_STAGES * WG_STAGE_BYTES + 256;
 
-__global__ void __launch_bounds__(256, 1)
-wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ CUtensorMap tmX, const WgradParams p) {
+__global__ void __launch_bounds__(WG_THREADS, 1)
+wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ CUtensorMap tmX, const WgradParams p) {
     pdl_launch_dependents();
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + WG_STAGES * WG_STAGE_BYTES);
     uint64_t* full_bar = bars;
     uint64_t* empty_bar = bars + WG_STAGES;
-    uint64_t* acc_full = empty_bar + WG_STAGES;
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(acc_full + 1);
     const int warp_idx = uniform_warp_idx(), lane = threadIdx.x & 31;
+    const int wg = warp_idx >> 2;
 
     // work decomposition: blockIdx.y -> (cout tile, cin tile, tap group); blockIdx.x -> pixel split
     int wy = blockIdx.y;
@@ -62,96 +63,96 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constant_
     const int pb0 = blockIdx.x * p.blocks_per_split;
     const int pb1 = min(p.num_pix_blocks, pb0 + p.blocks_per_split);
 
-    if (warp_idx == 0 && lane == 0) { tma_prefetch_desc(&tmDY); tma_prefetch_desc(&tmX); }
-    if (warp_idx == 1 && lane == 0) {
-        for (int i = 0; i < WG_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-        mbar_init(acc_full, 1);
+    if (warp_idx == 0 && lane == 0) {
+        tma_prefetch_desc(&tmDY);
+        tma_prefetch_desc(&tmX);
+        for (int i = 0; i < WG_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 2); }
         fence_barrier_init();
     }
-    if (warp_idx == 2) { tmem_alloc(tmem_ptr_smem, 256); tmem_relinquish(); }
-    pdl_wait();   // prologue above touched only smem / TMEM / kernel params
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
+    pdl_wait();   // the prologue above touched only shared memory and kernel parameters
 
-    if (warp_idx == 0) {
-        {   // whole warp converged; the *_e calls elect one lane for the instruction itself
+    if (wg == 0) {
+        setmaxnreg_dec<40>();
+        if (warp_idx == 0 && elect_one_sync()) {
             int stage = 0; uint32_t phase = 0;
             for (int pb = pb0; pb < pb1; ++pb) {
                 const int tw = pb % p.tiles_w, th = (pb / p.tiles_w) % p.tiles_h, tn = pb / (p.tiles_w * p.tiles_h);
                 mbar_wait(&empty_bar[stage], phase ^ 1);
-                mbar_arrive_expect_tx_e(&full_bar[stage], WG_A_BYTES + ntaps * WG_B_BYTES);
+                mbar_arrive_expect_tx(&full_bar[stage], WG_A_BYTES + ntaps * WG_B_BYTES);
                 uint8_t* sa = smem + stage * WG_STAGE_BYTES;
                 for (int c = 0; c < 2; ++c)
-                    tma_load_4d_e(&tmDY, &full_bar[stage], sa + c * (128 * 128), cot * 128 + c * 64, tw * p.bw, th * p.bh, tn * p.bn);
+                    tma_load_4d(&tmDY, &full_bar[stage], sa + c * (128 * 128), cot * 128 + c * 64, tw * p.bw, th * p.bh, tn * p.bn);
                 for (int t = 0; t < ntaps; ++t) {
                     uint8_t* sb = sa + WG_A_BYTES + t * WG_B_BYTES;
                     const int tap = tap0 + t;
                     const int ky = (p.ksize == 3) ? tap / 3 : 1, kx = (p.ksize == 3) ? tap % 3 : 1;
                     if (p.mode != 2) {
-                        tma_load_4d_e(&tmX, &full_bar[stage], sb, cit * WG_NT, tw * p.bw + kx - 1, th * p.bh + ky - 1, tn * p.bn);
+                        tma_load_4d(&tmX, &full_bar[stage], sb, cit * WG_NT, tw * p.bw + kx - 1, th * p.bh + ky - 1, tn * p.bn);
                     } else {
                         const int iy = ky - p.pad_lo, ix = kx - p.pad_lo;
-                        tma_load_5d_e(&tmX, &full_bar[stage], sb, (ix & 1) * p.C_in_map + cit * WG_NT, tw * p.bw + (ix >> 1), iy & 1,
+                        tma_load_5d(&tmX, &full_bar[stage], sb, (ix & 1) * p.C_in_map + cit * WG_NT, tw * p.bw + (ix >> 1), iy & 1,
                                     th * p.bh + (iy >> 1), tn * p.bn);
                     }
                 }
                 if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
             }
         }
-    } else if (warp_idx == 1) {
-        {   // whole warp converged; the *_e calls elect one lane for the instruction itself
-            constexpr uint32_t idesc = make_idesc_bf16(128, WG_NT, 1, 1);   // A and B both MN-major
-            int stage = 0; uint32_t phase = 0;
-            bool first = true;
-            for (int pb = pb0; pb < pb1; ++pb) {
-                mbar_wait(&full_bar[stage], phase);
-                tc_fence_after();
-                const uint32_t sa = smem_u32(smem + stage * WG_STAGE_BYTES);
-                for (int t = 0; t < ntaps; ++t) {
-                    const uint32_t sb = sa + WG_A_BYTES + t * WG_B_BYTES;
+        return;
+    }
+
+    setmaxnreg_inc<232>();
+    // D[co, ci] (per tap) = dY^T X over the tile's 128 pixels: A = dY chunk (wg - 1), B = X tap tile, both MN-major
+    float acc[WG_TG][WG_NT / 2];
 #pragma unroll
-                    for (int kk = 0; kk < 8; ++kk) {   // 128 pixels = 8 x K16
-                        tc_mma_ss_e(tmem_base + t * WG_NT, make_smem_desc(sa + kk * 2048, 128 * 128, 1024, 2),
-                                  make_smem_desc(sb + kk * 2048, 128 * 128, 1024, 2), idesc, (first && kk == 0) ? 0u : 1u);
-                    }
+    for (int t = 0; t < WG_TG; ++t)
+#pragma unroll
+        for (int i = 0; i < WG_NT / 2; ++i) acc[t][i] = 0.f;
+    {
+        int stage = 0; uint32_t phase = 0;
+        for (int pb = pb0; pb < pb1; ++pb) {
+            mbar_wait(&full_bar[stage], phase);
+            const uint32_t sa = smem_u32(smem + stage * WG_STAGE_BYTES) + (wg - 1) * (128 * 128);
+            const uint32_t sb0 = smem_u32(smem + stage * WG_STAGE_BYTES) + WG_A_BYTES;
+            wgmma_fence();
+#pragma unroll
+            for (int t = 0; t < WG_TG; ++t) {
+                if (t < ntaps) {
+#pragma unroll
+                    for (int kk = 0; kk < 8; ++kk)   // 128 pixels = 8 x K16
+                        Wgmma<WG_NT, 1, 1>::mma(acc[t], make_smem_desc(sa + kk * 2048, 128 * 128, 1024, SWZ_128B),
+                                                make_smem_desc(sb0 + t * WG_B_BYTES + kk * 2048, 128 * 128, 1024, SWZ_128B), 1);
                 }
-                first = false;
-                tc_commit_e(&empty_bar[stage]);
-                if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
             }
-            tc_commit_e(acc_full);
+            wgmma_commit();
+            wgmma_wait<0>();
+            if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[stage]);
+            if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
         }
-    } else if (warp_idx >= 4) {
-        if (pb1 > pb0) {
-            mbar_wait(acc_full, 0);
-            tc_fence_after();
-            const int quad = warp_idx & 3;
-            const int co = cot * 128 + quad * 32 + lane;
-            const uint32_t lane_off = uint32_t(quad * 32) << 16;
-            const int kk2 = p.ksize * p.ksize;
-            for (int t = 0; t < ntaps; ++t) {
 #pragma unroll
-                for (int c = 0; c < WG_NT / 32; ++c) {
-                    uint32_t v[32];
-                    tmem_ld_32x32(tmem_base + lane_off + t * WG_NT + c * 32, v);
-                    tc_wait_ld();
-                    if (co < p.Cout) {
+        for (int t = 0; t < WG_TG; ++t) wgmma_fence_acc(acc[t]);
+    }
+    if (pb1 <= pb0) return;
+    // acc[t][j*4 + i*2 + c] = D[co row w*16 + lane/4 + 8i][ci col 8j + 2*(lane%4) + c]
+    const int w4 = warp_idx & 3, q = lane & 3;
+    const int kk2 = p.ksize * p.ksize;
 #pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            const int ci = cit * WG_NT + c * 32 + j;
-                            if (ci < p.Cin)
-                                atomicAdd(&p.dw[((long long)co * p.Cin + ci) * kk2 + tap0 + t], p.alpha * __uint_as_float(v[j]));
-                        }
-                    }
+    for (int i = 0; i < 2; ++i) {
+        const int co = cot * 128 + (wg - 1) * 64 + w4 * 16 + (lane >> 2) + 8 * i;
+        if (co >= p.Cout) continue;
+#pragma unroll
+        for (int t = 0; t < WG_TG; ++t) {
+            if (t >= ntaps) continue;
+#pragma unroll
+            for (int j = 0; j < WG_NT / 8; ++j)
+#pragma unroll
+                for (int c = 0; c < 2; ++c) {
+                    const int ci = cit * WG_NT + 8 * j + 2 * q + c;
+                    if (ci < p.Cin)
+                        atomicAdd(&p.dw[((long long)co * p.Cin + ci) * kk2 + tap0 + t], p.alpha * acc[t][j * 4 + i * 2 + c]);
                 }
-            }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp_idx == 2) { tc_fence_after(); tmem_dealloc(tmem_base, 256); }
 }
 
 // ---------------------------------------------------------------------------------------------- weight re-layout
@@ -358,10 +359,10 @@ extern "C" int cl_conv_wgrad(const void* dy, const void* x, float* dw, int n_img
     }
     static bool done = false;
     if (!done) {
-        CL_CUDA_CHECK(cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM));
+        CL_CUDA_CHECK(cudaFuncSetAttribute(wgrad_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM));
         done = true;
     }
-    launch_k(wgrad_tc_kernel, dim3(splits, tiles), 256, WG_SMEM, stream, tDY, tX, p);
+    launch_k(wgrad_wgmma_kernel, dim3(splits, tiles), WG_THREADS, WG_SMEM, stream, tDY, tX, p);
     DONE();
 }
 

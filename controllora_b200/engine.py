@@ -1,6 +1,6 @@
 """Tape-based execution engine for the UNet hot path.
 
-Every forward op launches sm_100a kernels through the C ABI and (when a tape is active) records a closure that launches
+Every forward op launches sm_90a kernels through the C ABI and (when a tape is active) records a closure that launches
 the backward kernels.  Gradients of frozen weights are never computed ("frozen-weight gradient path elided"): the
 backward emits only activation gradients (dX), LoRA dA/dB, and gradients w.r.t. the injected control states.
 

@@ -1,6 +1,6 @@
 """Execution of the ControlLoRA hint encoder (/root/reference/models.py:810-835: conv_in, the SimpleDownEncoderBlock2D
-pyramid, the per-level pre-LoRA 1x1 ConvBlock2D) on the B200 kernels, forward and backward.  Unlike the UNet these
-layers are trainable: the backward also produces dW (tcgen05 wgrad), dbias, dgamma, dbeta.
+pyramid, the per-level pre-LoRA 1x1 ConvBlock2D) on the CUDA kernels, forward and backward.  Unlike the UNet these
+layers are trainable: the backward also produces dW (wgmma wgrad), dbias, dgamma, dbeta.
 
 Activations are NHWC bf16; parameters stay fp32 nn.Parameters and are re-laid-out to bf16 GEMM operands every step.
 """

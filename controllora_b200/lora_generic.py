@@ -1,7 +1,7 @@
 """General adapter chains: every wiring of /root/reference/models.py:118-431 that the fused one-launch path (lora_runtime.py) does
 not cover, executed adapter by adapter in the reference's own order.
 
-The fused path packs a projection and all of its LoRA deltas into ONE tcgen05 GEMM, which needs every adapter to read the
+The fused path packs a projection and all of its LoRA deltas into ONE wgmma GEMM, which needs every adapter to read the
 projection's INPUT and the ranks to sum to <= 8.  The reference allows more (models.py:232-243, 248-265, 275-282, 366-426):
 
   * `post_add` adapters inside a stacked chain: adapter i reads the running projection output, i.e. the sum of the base
@@ -201,7 +201,7 @@ class ControlMLP:
     """`scale * to_control([h ; c])` of a concat_hidden processor (models.py:207-220 / 342-355) - or `to_control(c)` when the layer
     takes the control states alone - as a term that is either added to the hidden states (V2: h' = h + term) or handed out on its
     own.  Ranks <= DENSE_RANK: hi/lo skinny GEMMs + rank-8 updates (fp32-accurate rank space, like the fused V2 kernels); wider
-    control MLPs (danbooru-sketch's rank 256): dense bf16 GEMMs with tcgen05 weight gradients, like lora_runtime._v1cat_q."""
+    control MLPs (danbooru-sketch's rank 256): dense bf16 GEMMs with wgmma weight gradients, like lora_runtime._v1cat_q."""
 
     def __init__(self, layer, C: int, plan, grad_of, device, concat_hidden: bool):
         down, up = layer.down.weight, layer.up.weight

@@ -2,13 +2,13 @@
 /root/reference/models.py:72-431) onto fused kernel launches.
 
 For every attention layer the adapter chain [pre_loras..., processor, post_loras...] (models.py:232-243 etc.) is packed
-into one rank<=8 `LoraSlot` per projection, so a projection and all of its LoRA deltas are ONE tcgen05 GEMM launch.
+into one rank<=8 `LoraSlot` per projection, so a projection and all of its LoRA deltas are ONE wgmma GEMM launch.
 
 v1 control (models.py:237-238):  q = Wq h + s Bq Aq (h + s Bc Ac c)
         = Wq h + s Bq ( Aq h  +  s (Aq Bc) (Ac c) )               -> `t_add` of the fused GEMM epilogue,
   with u = Ac c computed for all processors of a UNet level by one GEMM over the level's control state.
 v1 control with `concat_hidden` (models.py:208-214; configs/danbooru-sketch.json, control_rank 256):
-        ctrl = s Bc Ac [h ; c]  is a real two-layer MLP, so it runs as dense tcgen05 GEMMs (Ac_h, Ac_c, Bc are trainable: their
+        ctrl = s Bc Ac [h ; c]  is a real two-layer MLP, so it runs as dense wgmma GEMMs (Ac_h, Ac_c, Bc are trainable: their
         weight gradients are dense GEMMs too), followed by the rank-4 `to_q_lora` on h + ctrl.
 V2 control (models.py:369, 415):  h' = h + s Bc Ac [h ; c]  is a rank-r update of the hidden states (before q/k/v and
   again before to_out), done by one skinny GEMM + one rank-update kernel.

@@ -1,4 +1,4 @@
-"""Drop-in class surface of /root/reference/models.py, backed by the B200 kernels.
+"""Drop-in class surface of /root/reference/models.py, backed by the CUDA kernels.
 
 Same class names, constructor kwargs, attribute names and state-dict keys as the reference (models.py:72-835), so the
 reference's configs/*.json and the wiring code of train_text_to_image_control_lora.py:469-487 work unchanged:

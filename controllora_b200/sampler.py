@@ -1,4 +1,4 @@
-"""Denoise loop on the B200 UNet: classifier-free guidance + DDIM (eta = 0) or DPM-Solver++(2M), the inference call
+"""Denoise loop on the CUDA UNet: classifier-free guidance + DDIM (eta = 0) or DPM-Solver++(2M), the inference call
 pattern of the reference (`StableDiffusionPipeline.__call__` as used at train_text_to_image_control_lora.py:829-843 and
 apps/gradio_canny2image.py:81-89; BASELINE config 3 = 50-step DDIM at batch 8 -> UNet batch 16; the reference swaps in
 `DPMSolverMultistepScheduler` for validation / the apps: train_text_to_image_control_lora.py:817-823,

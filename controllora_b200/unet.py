@@ -1,8 +1,8 @@
-"""B200-native SD-1.5 UNet (the frozen network that /root/reference/train_text_to_image_control_lora.py:782 calls as
+"""H100-native SD-1.5 UNet (the frozen network that /root/reference/train_text_to_image_control_lora.py:782 calls as
 `unet(noisy_latents, timesteps, encoder_hidden_states).sample`), built on the tape engine.
 
 Topology / parameter names follow diffusers 0.13 `UNet2DConditionModel` (state-dict compatible), the compute is ours:
-channels-last bf16 activations, every conv / linear on the tcgen05 GEMM, fused attention, fused norm kernels, and a
+channels-last bf16 activations, every conv / linear on the wgmma GEMM, fused attention, fused norm kernels, and a
 backward pass that only produces what ControlLoRA training needs (dX, LoRA dA/dB, d control-states).
 """
 from __future__ import annotations

@@ -1,9 +1,9 @@
-"""`AutoencoderKL` — the frozen SD-1.5 VAE either side of the hot path, on the same sm_100a kernels (SURVEY.md 8f rank 3):
+"""`AutoencoderKL` — the frozen SD-1.5 VAE either side of the hot path, on the same sm_90a kernels (SURVEY.md 8f rank 3):
 
   latents = vae.encode(pixel_values).latent_dist.sample() * vae.config.scaling_factor      train_text_to_image_control_lora.py:753-754
   image   = vae.decode(latents / vae.config.scaling_factor).sample                          StableDiffusionPipeline (…:829-843, apps/*)
 
-Forward only (the reference freezes the VAE, train_…:430).  Every conv runs on the tcgen05 implicit-GEMM kernel, the norms on
+Forward only (the reference freezes the VAE, train_…:430).  Every conv runs on the wgmma implicit-GEMM kernel, the norms on
 the GroupNorm kernels; the mid-block `AttentionBlock` has ONE head of width 512 (beyond the flash kernels' head-dim range), so
 it runs as GEMMs around a row-softmax kernel (scores in fp32).  The 1x1 `quant_conv` is folded into `encoder.conv_out`, the
 1x1 `post_quant_conv` into `decoder.conv_in` (exact: weight products; its bias becomes a per-channel shift of the latents).

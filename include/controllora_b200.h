@@ -1,4 +1,4 @@
-/* controllora_b200 — C ABI of the B200-native ControlLoRA UNet hot path.
+/* controllora_b200 — C ABI of the H100-native ControlLoRA UNet hot path.
  *
  * The reference (HighCWu/ControlLoRA) is pure Python: its "FFI" for this path is the set of torch/ATen calls
  * issued by diffusers' UNet2DConditionModel and by models.py's attention processors.  Each entry point below
@@ -35,7 +35,7 @@ int cl_version(void);
 int64_t cl_launch_count(void);
 
 /* ------------------------------------------------------------------------------------------------------------
- * K1/K4: tcgen05 GEMM  D[M,N] = epilogue( A[M,K] * B[N,K]^T )   (bf16 x bf16 -> fp32 in TMEM)
+ * K1/K4: wgmma GEMM  D[M,N] = epilogue( A[M,K] * B[N,K]^T )   (bf16 x bf16 -> fp32 accumulators)
  *
  * Replaces: attn.to_q/to_k/to_v/to_out[0] + LoRALinearLayer side path  (models.py:124-147, 231-282, 373-423),
  *           diffusers FeedForward linears, Transformer2DModel proj_in/proj_out (1x1 conv == GEMM on NHWC),
@@ -280,7 +280,7 @@ int cl_small_matmul(const float* a, int64_t sa_i, int64_t sa_j, const float* b, 
 /* ------------------------------------------------------------------------------------------------------------
  * K6: hint-encoder training support (the ControlLoRA conv stack of models.py:434-835 is trainable, so unlike the UNet
  * it needs weight gradients and a per-step re-layout of its fp32 master weights).
- *   cl_conv_wgrad:       dW[co,ci,ky,kx] += alpha * sum dY * X(shifted)   on tcgen05 (MN-major operands, split-K + RED)
+ *   cl_conv_wgrad:       dW[co,ci,ky,kx] += alpha * sum dY * X(shifted)   on wgmma (MN-major operands, split-K + RED)
  *   cl_conv_weight_prep: w fp32 [Cout][Cin][k][k] -> wf bf16 [Cout][k*k][Cin] (forward) and wd bf16 [Cin][k*k flipped][Cout] (dX)
  *   cl_colsum:           out[c] += alpha * sum_m x[m, c]                  (bias gradients)
  *   cl_conv_in_wgrad:    weight gradient of the 3-channel conv_in (SIMT)

@@ -340,9 +340,9 @@ def accumulate_case(B=2, HW=16, micro=3):
 
 
 def resume_case(B=2, HW=16):
-    """Resume equivalence (train_text_to_image_control_lora.py:713-735 / 805-809): 3 steps in one run == 2 steps, save_checkpoint, a
-    NEW Trainer on freshly initialised models, load_checkpoint, 1 more step - bit for bit (parameters, AdamW moments, device step
-    counter, and the device Philox counter: step 3 draws the same noise / timesteps in both runs)."""
+    """Resume equivalence (train_text_to_image_control_lora.py:713-735 / 805-809): 2 steps, save_checkpoint, a NEW Trainer on freshly
+    initialised models, load_checkpoint restores parameters and AdamW moments bit for bit, and 1 more step on both gives the same
+    result (parameters, AdamW moments, device step counter, and the device Philox counter: step 3 draws the same noise / timesteps)."""
     import tempfile
 
     import torch
@@ -363,29 +363,29 @@ def resume_case(B=2, HW=16):
     batches = [((0.2 * torch.randn(B, 4, HW, HW, generator=g)).to(DEV), torch.randn(B, 77, 64, generator=g).to(torch.bfloat16).to(DEV),
                 (torch.rand(B, 3, HW * 8, HW * 8, generator=g) * 2 - 1).to(DEV)) for _ in range(3)]
     a, _ = make(0)
-    for b in batches:
-        loss_a = a.step_from_latents(*b)
-    draw_a = [t.detach().cpu().clone() for t in a.last_noise_draw]
-    b1, _ = make(0)
     for b in batches[:2]:
-        b1.step_from_latents(*b)
+        a.step_from_latents(*b)
     with tempfile.TemporaryDirectory() as d:
-        path = b1.save_checkpoint(d)
+        path = a.save_checkpoint(d)
         b2, _ = make(5)                                   # different initial weights: everything must come from the checkpoint
         gs = b2.load_checkpoint(path)
+    restored = all(torch.equal(x, y) for x, y in ((a.flat_p, b2.flat_p), (a.flat_m, b2.flat_m), (a.flat_v, b2.flat_v)))
+    loss_a = a.step_from_latents(*batches[2])
+    draw_a = [t.detach().cpu().clone() for t in a.last_noise_draw]
     loss_b = b2.step_from_latents(*batches[2])
     if DEV == "cuda":
         torch.cuda.synchronize()
     draw_b = [t.detach().cpu().clone() for t in b2.last_noise_draw]
     # CPU host-logic mode is deterministic: bit for bit.  On the GPU the weight-gradient kernels reduce with fp32 atomics (split-K +
-    # RED, csrc/wgrad.cu), so two RUNS differ at the 1e-7 level even without a checkpoint in between (and Adam turns gradient noise of
-    # true-zero gradients into +-lr steps): same tolerance as the eager-vs-graph comparison (2e-3).  The restored counters and the
-    # step-3 noise draw are exact on both.
+    # RED, csrc/wgrad.cu), so two executions of the same step differ at the 1e-7 level (and Adam turns gradient noise of true-zero
+    # gradients into +-lr steps; over several steps the two trajectories drift apart by far more, which is why both sides start the
+    # compared step from the same restored state): same tolerance as the eager-vs-graph comparison (2e-3).  The restored state,
+    # the restored counters and the step-3 noise draw are exact on both.
     if DEV == "cuda":
         close = lambda x, y: float((x - y).norm() / (y.norm() + 1e-30)) < 2e-3
     else:
         close = torch.equal
-    same = {"global_step": gs == 2, "params": close(a.flat_p, b2.flat_p), "exp_avg": close(a.flat_m, b2.flat_m),
+    same = {"global_step": gs == 2, "restored": restored, "params": close(a.flat_p, b2.flat_p), "exp_avg": close(a.flat_m, b2.flat_m),
             "exp_avg_sq": close(a.flat_v, b2.flat_v), "step": a.step_idx == b2.step_idx == int(b2.step_dev) == 3,
             "rng_counter": int(a.rng_counter) == int(b2.rng_counter) == 3,
             "loss": abs(float(loss_a) - float(loss_b)) <= (2e-3 * abs(float(loss_a)) if DEV == "cuda" else 0.0),

@@ -1,4 +1,4 @@
-"""GPU parity of the B200 UNet (fwd + bwd) against the fp32 CPU oracle on a tiny SD-style config.
+"""GPU parity of the CUDA UNet (fwd + bwd) against the fp32 CPU oracle on a tiny SD-style config.
 
 usage: python tests/check_unet.py [plain|v1|v2|v1_stacked|v1_post_add|v1_concat|none] ...   (default: all, each in a subprocess)
 """

@@ -52,7 +52,7 @@ def gemm(a, b, *, out=None, bias=None, row_bias=None, rows_per_group=0, residual
          lora_scale=1.0, t_add=None, t_out=None, out_fp32=False, conv_stride=0, pad_lo=1, block_n=0):
     assert a.dtype == BF16 and b.dtype == BF16
     N, K = b.shape
-    # the argument checks of cl_gemm (csrc/gemm.cu): a host program the kernel would reject must fail here too
+    # the argument checks of cl_gemm (csrc/gemm_wgmma.cu): a host program the kernel would reject must fail here too
     assert N % 4 == 0 and K % 8 == 0 and b.stride(0) % 8 == 0 and b.stride(1) == 1, "cl_gemm: N % 4, K % 8, ldb % 8"
     assert (ext is None) == (lora_up is None) and (lora_up is not None or (t_add is None and t_out is None))
     if lora_up is not None:

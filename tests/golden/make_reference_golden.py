@@ -104,20 +104,39 @@ def run_front_half(M, case):
         for n, p in op.named_parameters():
             if p.grad is not None:
                 small[f"pre_lora::{name}::{n}"] = p.grad.detach().clone()
-    # one flat tensor + an index per dictionary (a pickle of ~1000 tiny tensors is mostly per-tensor overhead)
+    # one flat tensor + an index per dictionary (a pickle of ~1000 tiny tensors is mostly per-tensor overhead); a tensor larger
+    # than SAMPLE elements is kept as the fixed, seeded sample `sample(t)` (keeps the file under 1 MB), its full norm beside it
     out["grads"] = {"names": list(small), "shapes": [tuple(v.shape) for v in small.values()],
-                    "flat": torch.cat([v.reshape(-1) for v in small.values()])}
+                    "flat": torch.cat([sample(v) for v in small.values()]),
+                    "norms": torch.stack([v.double().norm().float() for v in small.values()])}
     out["grad_norms"] = {"names": list(norms), "values": torch.stack(list(norms.values()))}
     return out
 
 
+SAMPLE = 96
+
+
+def sample_index(numel: int) -> torch.Tensor:
+    """Fixed, seeded element indices of a flattened tensor (all of them up to SAMPLE elements)."""
+    if numel <= SAMPLE:
+        return torch.arange(numel)
+    return torch.randperm(numel, generator=torch.Generator().manual_seed(numel))[:SAMPLE].sort().values
+
+
+def sample(t: torch.Tensor) -> torch.Tensor:
+    t = t.detach().float().cpu().reshape(-1)
+    return t[sample_index(t.numel())].clone()
+
+
 def unpack_grads(packed) -> dict:
+    """name -> the stored sample of that gradient (compare with `sample(tensor)`)."""
     out, off = {}, 0
     for n, shp in zip(packed["names"], packed["shapes"]):
         k = 1
         for d in shp:
             k *= d
-        out[n] = packed["flat"][off:off + k].view(shp)
+        k = min(k, SAMPLE)
+        out[n] = packed["flat"][off:off + k]
         off += k
     return out
 

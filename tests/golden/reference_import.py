@@ -25,7 +25,10 @@ REFERENCE_ROOT = Path("/root/reference")
 
 
 def available() -> bool:
-    return (REFERENCE_ROOT / "models.py").is_file()
+    try:
+        return (REFERENCE_ROOT / "models.py").is_file()
+    except OSError:        # e.g. a parent directory this user may not enter
+        return False
 
 
 class LoRALinearLayer(nn.Module):

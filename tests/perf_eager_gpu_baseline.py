@@ -4,8 +4,8 @@ train_text_to_image_control_lora.py:437-447) — using the oracle restatement (o
 installable here.  SURVEY.md §8(d) calls this "the real bar": the reference has no kernels of its own.
 
 This is a measurement script kept with the tests (it executes the oracle, which only tests/, smoke() and the CPU arm of
-bench.py may do); it is not collected by pytest, not part of the product path and not part of bench.py's JSON line.  Its
-output goes to profiles/.   usage: python tests/perf_eager_gpu_baseline.py [--batch 8] [--steps 5] [--config diffusiondb-canny-v2]
+bench.py may do); it is not collected by pytest, not part of the product path and not part of bench.py's JSON line.  It
+prints one JSON line.   usage: python tests/perf_eager_gpu_baseline.py [--batch 8] [--steps 5] [--config diffusiondb-canny-v2]
 """
 import argparse
 import json

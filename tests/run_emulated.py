@@ -1,6 +1,6 @@
 """Runs the parity checkers (tests/check_*.py) in host-logic mode: CLB_EMU=1, every kernel wrapper replaced by its torch
 restatement (tests/emu_ops.py), everything above the C ABI - tape engine, LoRA slot packing, control algebra, hint-encoder
-program, Trainer - is the product code and is compared with the fp32 oracle exactly as the `-m gpu` suite does on a B200.
+program, Trainer - is the product code and is compared with the fp32 oracle exactly as the `-m gpu` suite does on an H100.
 
 usage: python tests/run_emulated.py [case ...]      (prints one `RESULT <case> OK|FAIL <seconds>` line per case)
 Must be its own process: the mode is chosen when the first checker is imported (tests/_device.py)."""

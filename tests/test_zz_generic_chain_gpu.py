@@ -1,4 +1,4 @@
-"""B200 tests added after the last GPU run of round 2 (the same cases pass in host-logic mode on the CPU, tests/test_host_emulated.py, where
+"""GPU tests of step-level features and the general adapter chains (the same cases pass in host-logic mode on the CPU, tests/test_host_emulated.py, where
 every launch also goes through the real launchers' argument validation).  Ordered from the paths built on kernels / call patterns that earlier
 GPU runs already exercised to the newest code, so that `pytest -x` reports as much as possible:
   1. the CUDA path against golden vectors computed by the reference's own models.py (fused path, tests/check_reference_golden.py)

@@ -76,10 +76,10 @@ def plain_bn256():
 
 @case
 def plain_bn320():
-    """256 x 320 CTA-pair tiles (two 160-column MMAs per k-step sharing the A stage, one accumulator buffer)."""
+    """requested 320-column tiles (not an instantiated width: cl_gemm falls back to its tail-tile choice), M tails included."""
     _run_plain(4096, 640, 2560, 320)
     _run_plain(32768, 320, 2880, 320)
-    _run_plain(1000, 320, 2048, 320)      # M tail inside a pair
+    _run_plain(1000, 320, 2048, 320)      # M tail
 
 
 @case
@@ -246,7 +246,7 @@ def conv_s2():
 
 @case
 def conv_bn320():
-    """deep-K convs whose N is a multiple of 320 take the 256 x 320 pair tile (plan_tiles); with the fused epilogue operands"""
+    """deep-K convs whose N is a multiple of 320, with the fused epilogue operands"""
     _conv_case(8, 64, 64, 320, 320, 1, 1, True)
     _conv_case(8, 32, 32, 640, 640, 1, 1, True)
     _conv_case(8, 32, 32, 1280, 640, 1, 1, False)

@@ -1,4 +1,4 @@
-"""Denoise-loop timing on the B200 UNet for the two inference call patterns of the reference (synthetic weights / inputs):
+"""Denoise-loop timing on the CUDA UNet for the two inference call patterns of the reference (synthetic weights / inputs):
 
   c3   SURVEY §8(d) config 3: v1 ControlLoRA (mpii-pose architecture), 512x512, batch 8 (UNet batch 16 under CFG),
        50-step DDIM, guidance 7.5                                  (apps/gradio_*2image.py, train_...:829-843)

@@ -11,7 +11,7 @@ for (M, N, K) in shapes:
     b = (torch.randn(N, K, device="cuda") / K ** 0.5).to(torch.bfloat16)
     out = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
     res = []
-    for bn in (0, 64, 128, 160, 256, 320):
+    for bn in (0, 64, 128, 160, 256):
         if bn and N % bn:
             continue
         try:
