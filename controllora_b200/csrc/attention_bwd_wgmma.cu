@@ -16,7 +16,6 @@
 
 #include "common.cuh"
 #include "attention_tile.cuh"
-#define CLB_FAMILY 2      // CLB_PDL_MASK bit of this file's kernels
 #include "host_common.h"
 #include "../../include/controllora_b200.h"
 

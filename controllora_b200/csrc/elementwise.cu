@@ -4,7 +4,6 @@
 #include <stdio.h>
 
 #include "common.cuh"
-#define CLB_FAMILY 16      // CLB_PDL_MASK bit of this file's kernels
 #include "host_common.h"
 #include "../../include/controllora_b200.h"
 

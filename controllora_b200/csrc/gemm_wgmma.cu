@@ -20,7 +20,6 @@
 
 #include "common.cuh"
 #include "wgmma.cuh"
-#define CLB_FAMILY 1      // CLB_PDL_MASK bit of this file's kernels
 #include "host_common.h"
 #include "../../include/controllora_b200.h"
 
@@ -334,11 +333,11 @@ static int launch_gemm(const CUtensorMap& tA, const CUtensorMap& tB, const CUten
         CL_CUDA_CHECK(cudaFuncSetAttribute(gemm_wgmma_kernel<BN, EXT, BK>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
         attr_done = true;
     }
-    launch_k(gemm_wgmma_kernel<BN, EXT, BK>, (unsigned)grid, NUM_THREADS, smem_bytes, stream, tA, tB, tE, p, stages);
+    launch_k_pdl(gemm_wgmma_kernel<BN, EXT, BK>, (unsigned)grid, NUM_THREADS, smem_bytes, stream, tA, tB, tE, p, stages);
     count_launch();
     if (p.splits > 1) {
         const long long quads = (long long)p.M * (p.N / 4);
-        launch_k(splitk_finish_kernel, (unsigned)((quads + 255) / 256), 256, 0, stream,
+        launch_k_pdl(splitk_finish_kernel, (unsigned)((quads + 255) / 256), 256, 0, stream,
             p.split_ws, p.splits, p.M, p.N, full.bias, full.row_bias, full.rows_per_group, full.ld_rb, full.residual,
             full.ldr, full.out, full.ldd, full.out_fp32);
         count_launch();

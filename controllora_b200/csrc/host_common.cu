@@ -2,7 +2,6 @@
 
 #include <stdarg.h>
 #include <stdio.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include <atomic>
@@ -24,15 +23,6 @@ int set_error(int code, const char* fmt, ...) {
 }
 
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
-
-bool pdl_enabled(int family) {
-    // Programmatic dependent launch.  A dependent grid that starts while its predecessor drains lands on the SMs that free up
-    // first; kernels with several CTAs per SM then pile onto those SMs and run unbalanced, so only the GEMM (one CTA per SM, whose
-    // prologue - barrier init, descriptor prefetch - is what gets hidden) carries the attribute by default.  CLB_PDL=0 disables, CLB_PDL_MASK selects other families (bits: see host_common.h).
-    static const bool on = [] { const char* e = getenv("CLB_PDL"); return !(e && e[0] == '0'); }();
-    static const int mask = [] { const char* e = getenv("CLB_PDL_MASK"); return e ? atoi(e) : 1; }();
-    return on && (mask & family) != 0;
-}
 
 int num_sms() {
     static int sms = 0;
@@ -116,5 +106,5 @@ int get_tensor_map(CUtensorMap* out, const void* ptr, int rank, const uint64_t* 
 }  // namespace clb
 
 extern "C" const char* cl_last_error(void) { return clb::g_err; }
-extern "C" int cl_version(void) { return 100; }
+extern "C" int cl_version(void) { return 101; }
 extern "C" int64_t cl_launch_count(void) { return clb::g_launches.load(); }

@@ -18,30 +18,30 @@ int num_sms();
 int get_tensor_map(CUtensorMap* out, const void* ptr, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                    const uint32_t* box, int swizzle_bytes /* 0, 64 or 128 */);
 
-// Programmatic dependent launch (default: GEMM family only; CLB_PDL=0 disables): see pdl_launch_dependents / pdl_wait in common.cuh.
-// family: the CLB_FAMILY bit of the launching file (gemm 1, attention 2, norm 4, lora 8, elementwise 16, smallops 32, wgrad 64,
-// noise / optim 128); CLB_PDL_MASK (default: 1 = gemm, see host_common.cu) selects which families' kernels may start early.
-bool pdl_enabled(int family);
-#ifndef CLB_FAMILY
-#define CLB_FAMILY 128
-#endif
-
-// Launch `kernel` with the programmatic-stream-serialization attribute: inside a stream (or a captured CUDA graph) the
-// grid may start while the previous kernel drains; every kernel of this library executes griddepcontrol.wait before its
-// first global-memory access.  A launch error is left in cudaGetLastError() for the caller's check.
+// Launch `kernel` on `stream`.  A launch error is left in cudaGetLastError() for the caller's check.
 template <typename... KArgs, typename... Args>
 static inline void launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
+    kernel<<<grid, block, smem, stream>>>(static_cast<KArgs>(args)...);
+}
+
+// As launch_k, with the programmatic-stream-serialization attribute: inside a stream (or a captured CUDA graph) the grid
+// may start while the previous kernel drains; every kernel of this library executes griddepcontrol.wait (pdl_wait in
+// common.cuh) before its first global-memory access.  Only the GEMM launches use it.  A dependent grid that starts early
+// lands on the SMs that free up first; kernels with several CTAs per SM then pile onto those SMs and run unbalanced.  The
+// GEMM runs one CTA per SM, and what the early start hides is its prologue (barrier init, descriptor prefetch).
+template <typename... KArgs, typename... Args>
+static inline void launch_k_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = grid;
     cfg.blockDim = block;
     cfg.dynamicSmemBytes = smem;
     cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled(CLB_FAMILY) ? 1 : 0;
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr.val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
     (void)cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 

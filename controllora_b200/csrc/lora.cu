@@ -4,7 +4,6 @@
 #include <stdio.h>
 
 #include "common.cuh"
-#define CLB_FAMILY 8      // CLB_PDL_MASK bit of this file's kernels
 #include "host_common.h"
 #include "../../include/controllora_b200.h"
 
@@ -707,8 +706,7 @@ extern "C" int cl_v2_inject_bwd(const void* dy, const float* up, const float* do
     const size_t smem = (size_t)Ccols * 8 * sizeof(float);
     int blocks = (M + 15) / 16;
     // two 256-thread CTAs are resident per SM (registers): a grid beyond that only repeats the per-CTA table load
-    static const int v2_per_sm = [] { const char* e = getenv("CLB_V2_CTAS_PER_SM"); const int v = e ? atoi(e) : 2; return v < 1 ? 1 : v; }();
-    if (blocks > num_sms() * v2_per_sm) blocks = num_sms() * v2_per_sm;
+    if (blocks > num_sms() * 2) blocks = num_sms() * 2;
     const __nv_bfloat16* dd = reinterpret_cast<const __nv_bfloat16*>(dy);
     __nv_bfloat16* hh = reinterpret_cast<__nv_bfloat16*>(dh);
     if (Ccols <= 512) launch_k(v2_inject_bwd_kernel<2, 4>, blocks, 256, smem, stream, dd, up, down, alpha, dt_out, hh, M, Ccols, nullptr, 0, 0);
@@ -725,8 +723,7 @@ extern "C" int cl_rank4_project_update(const void* x, const float* proj, const f
     const size_t smem = (size_t)Ccols * 8 * sizeof(float);
     int blocks = (M + 15) / 16;
     // two 256-thread CTAs are resident per SM (registers): a grid beyond that only repeats the per-CTA table load
-    static const int v2_per_sm = [] { const char* e = getenv("CLB_V2_CTAS_PER_SM"); const int v = e ? atoi(e) : 2; return v < 1 ? 1 : v; }();
-    if (blocks > num_sms() * v2_per_sm) blocks = num_sms() * v2_per_sm;
+    if (blocks > num_sms() * 2) blocks = num_sms() * 2;
     const __nv_bfloat16* xx = reinterpret_cast<const __nv_bfloat16*>(x);
     __nv_bfloat16* yy = reinterpret_cast<__nv_bfloat16*>(y);
     if (Ccols <= 512) launch_k(v2_inject_bwd_kernel<2, 4>, blocks, 256, smem, stream, xx, proj, upd, alpha, t_out, yy, M, Ccols, uc, ldu, rc);

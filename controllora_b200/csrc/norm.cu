@@ -5,17 +5,10 @@
 #include <stdio.h>
 
 #include "common.cuh"
-#define CLB_FAMILY 4      // CLB_PDL_MASK bit of this file's kernels
 #include "host_common.h"
 #include "../../include/controllora_b200.h"
 
 namespace clb {
-
-__device__ __forceinline__ float silu_f(float z) { return z / (1.f + __expf(-z)); }
-__device__ __forceinline__ float silu_grad_f(float z) {
-    const float s = 1.f / (1.f + __expf(-z));
-    return s * (1.f + z * (1.f - s));
-}
 
 __device__ __forceinline__ void load8(const __nv_bfloat16* p, float (&f)[8]) {
     const uint4 u = *reinterpret_cast<const uint4*>(p);
@@ -29,26 +22,10 @@ __device__ __forceinline__ void store8(__nv_bfloat16* p, const float (&f)[8]) {
     *reinterpret_cast<uint4*>(p) = u;
 }
 
-// ---------------------------------------------------------------------------------------------- GroupNorm
-// Layout: x [n, HW, C]; group g = channels [g*cpg, (g+1)*cpg).  Three phases per direction, all HBM-bound:
-//   reduce   a CTA owns a slab of rows of one image, thread t always handles the same 8-channel chunk (blockDim.x is a
-//            multiple of C/8) so per-channel partial sums stay in registers; 2 CTAs per SM, 2 rows in flight per thread
-//   coef     one tiny kernel turns the sums into per-(image, channel) affine coefficient arrays
-//   apply    a flat, high-occupancy elementwise pass: one 16-byte chunk per thread-iteration, coefficients read as
-//            float4 from the (L1-resident) arrays (a slab variant with register-resident coefficients fits only one 480-thread CTA
-//            per SM).
-// Scratch `ws` (cl_groupnorm_ws_bytes): [n*G*2 fp64 group sums][4 x n*C fp32 coefficients][2 x n*C fp32 channel sums].
-
-static constexpr int GN_MAX_CHUNKS = 512;  // C <= 4096
-
 __device__ __forceinline__ uint4 ldg16(const __nv_bfloat16* p) { return __ldg(reinterpret_cast<const uint4*>(p)); }
 __device__ __forceinline__ void unpack8(const uint4& u, float (&f)[8]) {
     float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y), c = unpack_bf16x2(u.z), d = unpack_bf16x2(u.w);
     f[0] = a.x; f[1] = a.y; f[2] = b.x; f[3] = b.y; f[4] = c.x; f[5] = c.y; f[6] = d.x; f[7] = d.y;
-}
-__device__ __forceinline__ void ldg8f(const float* p, float (&f)[8]) {
-    const float4 a = __ldg(reinterpret_cast<const float4*>(p)), b = __ldg(reinterpret_cast<const float4*>(p + 4));
-    f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
 }
 __device__ __forceinline__ float fast_sigmoid(float z) { return __fdividef(1.f, 1.f + __expf(-z)); }
 __device__ __forceinline__ float silu_grad_fast(float z) {
@@ -56,280 +33,12 @@ __device__ __forceinline__ float silu_grad_fast(float z) {
     return s * (1.f + z * (1.f - s));
 }
 
-// mode 0: forward statistics   -> gsum[(n*G+g)*2 + {0,1}] += {sum x, sum x^2}                 (fp64 atomics)
-// mode 1: backward reductions  -> csum[0][n][c] += sum dz*x,  csum[1][n][c] += sum dz          (fp32 atomics)
-//         with dz = dy * silu'(x*sc + sh) when silu (sc = rstd*gamma, sh = beta - mean*sc), else dz = dy.
-template <int MODE>
-__global__ void __launch_bounds__(512, 2)
-gn_reduce_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ dy,
-                 const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ stats,
-                 double* __restrict__ gsum, float* __restrict__ csum, int n_img, int HW, int C, int G, int rows_per_cta,
-                 int silu) {
-    pdl_launch_dependents();
-    pdl_wait();
-    const int n = blockIdx.y;
-    const int chunks = C / 8;
-    const int cpg = C / G;
-    const int rows_par = blockDim.x / chunks;      // rows processed per iteration
-    const int chunk = threadIdx.x % chunks;
-    const int rsub = threadIdx.x / chunks;
-    const int row0 = blockIdx.x * rows_per_cta;
-    const int row1 = min(HW, row0 + rows_per_cta);
-    const bool active = rsub < rows_par;
-    const int c0 = chunk * 8;
-
-    float a0[8], a1[8];  // MODE 0: sum, sumsq.  MODE 1: sum dz*x, sum dz
-    float sc[8], sh[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) { a0[j] = a1[j] = 0.f; sc[j] = sh[j] = 0.f; }
-    if (MODE == 1 && silu && active) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const int g = (c0 + j) / cpg;
-            const float mu = stats[(n * G + g) * 2], rs = stats[(n * G + g) * 2 + 1];
-            sc[j] = rs * gamma[c0 + j];
-            sh[j] = fmaf(-mu, sc[j], beta[c0 + j]);
-        }
-    }
-    if (active) {
-        const __nv_bfloat16* xp = x + (long long)n * HW * C + c0;
-        const __nv_bfloat16* dp = dy + (long long)n * HW * C + c0;
-        // 2 rows in flight per thread; rows past the slab are clamped for the load and skipped for the sums
-        for (int r = row0 + rsub; r < row1; r += 2 * rows_par) {
-            const int r1 = r + rows_par;
-            const bool ok1 = r1 < row1;
-            const long long o0 = (long long)r * C, o1 = (long long)(ok1 ? r1 : r) * C;
-            if (MODE == 0) {
-                const uint4 u0 = ldg16(xp + o0), u1 = ldg16(xp + o1);
-                float xv[8];
-                unpack8(u0, xv);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) { a0[j] += xv[j]; a1[j] = fmaf(xv[j], xv[j], a1[j]); }
-                if (ok1) {
-                    unpack8(u1, xv);
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) { a0[j] += xv[j]; a1[j] = fmaf(xv[j], xv[j], a1[j]); }
-                }
-            } else {
-                const uint4 ux0 = ldg16(xp + o0), ud0 = ldg16(dp + o0), ux1 = ldg16(xp + o1), ud1 = ldg16(dp + o1);
-                float xv[8], dv[8];
-                unpack8(ux0, xv);
-                unpack8(ud0, dv);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    float dz = dv[j];
-                    if (silu) dz *= silu_grad_fast(fmaf(xv[j], sc[j], sh[j]));
-                    a0[j] = fmaf(dz, xv[j], a0[j]);
-                    a1[j] += dz;
-                }
-                if (ok1) {
-                    unpack8(ux1, xv);
-                    unpack8(ud1, dv);
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        float dz = dv[j];
-                        if (silu) dz *= silu_grad_fast(fmaf(xv[j], sc[j], sh[j]));
-                        a0[j] = fmaf(dz, xv[j], a0[j]);
-                        a1[j] += dz;
-                    }
-                }
-            }
-        }
-    }
-    // combine without shared-memory atomics (ATOMS costs ~2 cycles per lane): every row-group stores its per-channel
-    // partials, then the CTA sums them per channel.
-    extern __shared__ float gsh[];                        // [2][rows_par + 1][C]
-    float* part0 = gsh;                                   // [rows_par][C]
-    float* part1 = gsh + (size_t)rows_par * C;            // [rows_par][C]
-    float* tot0 = gsh + (size_t)2 * rows_par * C;         // [C]
-    float* tot1 = tot0 + C;
-    if (active) {
-        float* d0 = part0 + (size_t)rsub * C + c0;
-        float* d1 = part1 + (size_t)rsub * C + c0;
-        *reinterpret_cast<float4*>(d0) = make_float4(a0[0], a0[1], a0[2], a0[3]);
-        *reinterpret_cast<float4*>(d0 + 4) = make_float4(a0[4], a0[5], a0[6], a0[7]);
-        *reinterpret_cast<float4*>(d1) = make_float4(a1[0], a1[1], a1[2], a1[3]);
-        *reinterpret_cast<float4*>(d1 + 4) = make_float4(a1[4], a1[5], a1[6], a1[7]);
-    }
-    __syncthreads();
-    for (int c = threadIdx.x; c < C; c += blockDim.x) {
-        float s0 = 0.f, s1 = 0.f;
-        for (int g = 0; g < rows_par; ++g) { s0 += part0[(size_t)g * C + c]; s1 += part1[(size_t)g * C + c]; }
-        if (MODE == 0) { tot0[c] = s0; tot1[c] = s1; }
-        else {
-            atomicAdd(&csum[(size_t)n * C + c], s0);
-            atomicAdd(&csum[(size_t)(n_img + n) * C + c], s1);
-        }
-    }
-    if (MODE == 0) {
-        __syncthreads();
-        for (int g = threadIdx.x; g < G; g += blockDim.x) {
-            double s0 = 0.0, s1 = 0.0;
-            for (int c = g * cpg; c < (g + 1) * cpg; ++c) { s0 += tot0[c]; s1 += tot1[c]; }
-            atomicAdd(&gsum[(n * G + g) * 2], s0);
-            atomicAdd(&gsum[(n * G + g) * 2 + 1], s1);
-        }
-    }
-}
-
-// forward coefficients: stats {mean, rstd} per (image, group) and  y = x*sc + sh  per (image, channel).
-// coef layout: [4][n][C]; forward uses planes 0 (sc) and 1 (sh).
-__global__ void gn_fwd_coef_kernel(const double* __restrict__ gsum, const float* __restrict__ gamma,
-                                   const float* __restrict__ beta, float* __restrict__ stats, float* __restrict__ coef,
-                                   int n_img, int C, int G, double inv_m, float eps) {
-    pdl_launch_dependents();
-    pdl_wait();
-    const int n = blockIdx.x;
-    const int cpg = C / G;
-    for (int c = threadIdx.x; c < C; c += blockDim.x) {
-        const int g = c / cpg;
-        const double mu = gsum[(n * G + g) * 2] * inv_m;
-        double var = gsum[(n * G + g) * 2 + 1] * inv_m - mu * mu;
-        if (var < 0.0) var = 0.0;
-        const float rs = (float)(1.0 / sqrt(var + (double)eps));
-        const float fmu = (float)mu;
-        if (c == g * cpg) { stats[(n * G + g) * 2] = fmu; stats[(n * G + g) * 2 + 1] = rs; }
-        const float sc = rs * gamma[c];
-        coef[(size_t)n * C + c] = sc;
-        coef[(size_t)(n_img + n) * C + c] = fmaf(-fmu, sc, beta[c]);
-    }
-}
-
-// y = act(x*sc + sh): flat pass, grid (blocks, n)
-__global__ void __launch_bounds__(256)
-gn_apply_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ coef, __nv_bfloat16* __restrict__ y,
-                int n_img, int HW, int C, int silu) {
-    pdl_launch_dependents();
-    pdl_wait();
-    const int n = blockIdx.y;
-    const int chunks = C / 8;
-    const int total = HW * chunks;                      // < 2^31: HW * C / 8
-    const __nv_bfloat16* xp = x + (long long)n * HW * C;
-    __nv_bfloat16* yp = y + (long long)n * HW * C;
-    const float* scp = coef + (size_t)n * C;
-    const float* shp = coef + (size_t)(n_img + n) * C;
-    const int stride = gridDim.x * blockDim.x;
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += 2 * stride) {
-        const int i1 = i + stride;
-        const bool ok1 = i1 < total;
-        const uint4 u0 = ldg16(xp + (long long)i * 8);
-        const uint4 u1 = ldg16(xp + (long long)(ok1 ? i1 : i) * 8);
-        const int c0 = (i % chunks) * 8, c1 = ((ok1 ? i1 : i) % chunks) * 8;
-        float xv[8], sc[8], sh[8], o[8];
-        unpack8(u0, xv);
-        ldg8f(scp + c0, sc);
-        ldg8f(shp + c0, sh);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const float z = fmaf(xv[j], sc[j], sh[j]);
-            o[j] = silu ? z * fast_sigmoid(z) : z;
-        }
-        store8(yp + (long long)i * 8, o);
-        if (ok1) {
-            unpack8(u1, xv);
-            ldg8f(scp + c1, sc);
-            ldg8f(shp + c1, sh);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const float z = fmaf(xv[j], sc[j], sh[j]);
-                o[j] = silu ? z * fast_sigmoid(z) : z;
-            }
-            store8(yp + (long long)i1 * 8, o);
-        }
-    }
-}
-
-// backward coefficients, one CTA per image:  dx = dz*A - K1 - x*K2,  z = x*A + Bz  (planes 0..3 = A, Bz, K1, K2) from
-// the channel sums S1 = sum dz*x, S2 = sum dz:   sum dz*xhat = rstd*(S1 - mean*S2);   also dgamma / dbeta.
-__global__ void __launch_bounds__(512)
-gn_bwd_coef_kernel(const float* __restrict__ csum, const float* __restrict__ gamma, const float* __restrict__ beta,
-                   const float* __restrict__ stats, float* __restrict__ coef, float* __restrict__ dgamma,
-                   float* __restrict__ dbeta, int n_img, int C, int G, float inv_m) {
-    pdl_launch_dependents();
-    pdl_wait();
-    extern __shared__ float gs[];          // [2][G] group sums: sum dz*gamma, sum dz*gamma*xhat
-    const int n = blockIdx.x;
-    const int cpg = C / G;
-    for (int g = threadIdx.x; g < 2 * G; g += blockDim.x) gs[g] = 0.f;
-    __syncthreads();
-    for (int c = threadIdx.x; c < C; c += blockDim.x) {
-        const int g = c / cpg;
-        const float mu = stats[(n * G + g) * 2], rs = stats[(n * G + g) * 2 + 1];
-        const float s1 = csum[(size_t)n * C + c], s2 = csum[(size_t)(n_img + n) * C + c];
-        const float dzxh = rs * fmaf(-mu, s2, s1);          // sum dz*xhat of this channel
-        const float gm = gamma[c];
-        atomicAdd(&gs[g], gm * s2);
-        atomicAdd(&gs[G + g], gm * dzxh);
-        if (dgamma != nullptr) {
-            atomicAdd(&dgamma[c], dzxh);
-            atomicAdd(&dbeta[c], s2);
-        }
-    }
-    __syncthreads();
-    for (int c = threadIdx.x; c < C; c += blockDim.x) {
-        const int g = c / cpg;
-        const float mu = stats[(n * G + g) * 2], rs = stats[(n * G + g) * 2 + 1];
-        const float A = rs * gamma[c];
-        const float K2 = rs * rs * gs[G + g] * inv_m;
-        coef[(size_t)n * C + c] = A;
-        coef[(size_t)(n_img + n) * C + c] = fmaf(-mu, A, beta[c]);
-        coef[(size_t)(2 * n_img + n) * C + c] = fmaf(-mu, K2, rs * gs[g] * inv_m);
-        coef[(size_t)(3 * n_img + n) * C + c] = K2;
-    }
-}
-
-// dx (+)= dz*A - K1 - x*K2: flat pass, grid (blocks, n)
-__global__ void __launch_bounds__(256, 5)
-gn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ dy,
-                    const float* __restrict__ coef, __nv_bfloat16* __restrict__ dx, int n_img, int HW, int C, int silu,
-                    int accumulate) {
-    pdl_launch_dependents();
-    pdl_wait();
-    const int n = blockIdx.y;
-    const int chunks = C / 8;
-    const int total = HW * chunks;
-    const long long base = (long long)n * HW * C;
-    const float* Ap = coef + (size_t)n * C;
-    const float* Bp = coef + (size_t)(n_img + n) * C;
-    const float* K1p = coef + (size_t)(2 * n_img + n) * C;
-    const float* K2p = coef + (size_t)(3 * n_img + n) * C;
-    const int stride = gridDim.x * blockDim.x;
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
-        const uint4 ux = ldg16(x + base + (long long)i * 8), ud = ldg16(dy + base + (long long)i * 8);
-        const int c0 = (i % chunks) * 8;
-        float xv[8], dv[8], A[8], k[8], o[8];
-        unpack8(ux, xv);
-        unpack8(ud, dv);
-        ldg8f(Ap + c0, A);
-        if (silu) {
-            ldg8f(Bp + c0, k);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) dv[j] *= silu_grad_fast(fmaf(xv[j], A[j], k[j]));
-        }
-#pragma unroll
-        for (int j = 0; j < 8; ++j) o[j] = dv[j] * A[j];
-        ldg8f(K1p + c0, k);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) o[j] -= k[j];
-        ldg8f(K2p + c0, k);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) o[j] = fmaf(-xv[j], k[j], o[j]);
-        if (accumulate) {
-            float p[8];
-            load8(dx + base + (long long)i * 8, p);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) o[j] += p[j];
-        }
-        store8(dx + base + (long long)i * 8, o);
-    }
-}
-
-// ---------------------------------------------------------------------------------------------- GroupNorm, one launch
+// ---------------------------------------------------------------------------------------------- GroupNorm
+// Layout: x [n, HW, C]; group g = channels [g*cpg, (g+1)*cpg).  One launch per direction, no workspace.
 // One thread-block CLUSTER per image (up to 16 CTAs, each owning a slab of rows of all channels): phase 1 reduces the slab
 // (thread == fixed 8-channel chunk, partial sums in registers), the CTAs exchange their per-group partial sums through
 // distributed shared memory (fp64), every CTA derives the per-channel affine coefficients, and phase 2 streams the slab
-// again - from L2, where phase 1 just left it - to write y (forward) or dx (backward).  Replaces reduce -> memset ->
-// coef -> apply (3 kernels + 1 memset node, fp64 global atomics, a workspace) by ONE kernel and no workspace.
+// again - from L2, where phase 1 just left it - to write y (forward) or dx (backward).
 __device__ __forceinline__ double ld_dsmem_f64(uint32_t cluster_addr) {
     double v;
     asm volatile("ld.shared::cluster.f64 %0, [%1];" : "=d"(v) : "r"(cluster_addr) : "memory");
@@ -474,7 +183,7 @@ gn_cluster_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __re
     }
     // ---------------- exchange: every CTA sums the partials of all CTAs of its image (distributed shared memory)
     if (CL > 1) cluster_sync_all(); else __syncthreads();
-    double* gtot = reinterpret_cast<double*>(part0);                 // [G][2] (part0 is free now)
+    double* gtot = reinterpret_cast<double*>(part0);                 // [G][2] (part0 / part1 are free now; sized to hold it)
     for (int g = threadIdx.x; g < 2 * G; g += blockDim.x) {
         double s = 0.0;
         if (CL > 1) {
@@ -728,63 +437,46 @@ ln_bwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restri
 
 using namespace clb;
 
-static int gn_launch_geometry(int HW, int C, int n, int& threads, int& rows_per_cta, int& grid_x) {
-    const int chunks = C / 8;
-    if (C % 8 != 0 || chunks > GN_MAX_CHUNKS) return set_error(CL_ERR_UNSUPPORTED, "groupnorm: C must be a multiple of 8 and <= 4096");
-    int rows_par = 512 / chunks;
-    if (rows_par < 1) rows_par = 1;
-    threads = ((rows_par * chunks + 31) / 32) * 32;
-    if (threads > 512) { rows_par = 1; threads = ((chunks + 31) / 32) * 32; }
-    // ~4 CTAs per SM across the batch (2 resident at a time), but at least 4 row groups per CTA
-    int target_ctas = (num_sms() * 4 + n - 1) / n;
-    rows_per_cta = (HW + target_ctas - 1) / target_ctas;
-    if (rows_per_cta < 4 * rows_par) rows_per_cta = 4 * rows_par;
-    grid_x = (HW + rows_per_cta - 1) / rows_per_cta;
-    return CL_OK;
-}
-
-static int gn_flat_blocks(int HW, int C, int n, int per_thread) {
-    const long long total = (long long)HW * (C / 8);
-    long long blocks = (total + 256LL * per_thread - 1) / (256LL * per_thread);
-    const long long cap = ((long long)num_sms() * 16 + n - 1) / n;     // ~2 waves of 8 resident 256-thread CTAs per SM
-    if (blocks > cap) blocks = cap;
-    if (blocks < 1) blocks = 1;
-    return (int)blocks;
-}
-
-
-// One-launch GroupNorm: pick the cluster size (CTAs per image) and launch gn_cluster_kernel<BWD>.  Returns CL_OK, or a
-// positive value when this shape / device has to take the three-kernel path.
+// One-launch GroupNorm: pick the channel ranges and the cluster size (CTAs per image), launch gn_cluster_kernel<BWD>.
 template <int BWD>
 static int gn_cluster_launch(const __nv_bfloat16* x, const __nv_bfloat16* dy, const float* gamma, const float* beta, float* stats,
                              __nv_bfloat16* out, float* dgamma, float* dbeta, int n, int HW, int C, int G, float eps, int silu,
                              int accumulate, cudaStream_t stream) {
-    static const int enabled = [] { const char* e = getenv("CLB_GN_FUSED"); return (e && e[0] == '0') ? 0 : 1; }();
-    if (!enabled || C % 8 != 0 || C < 8 || C % G != 0) return 1;
+    static const char* c_msg = "groupnorm: C must be a multiple of 8 and <= 4096";
+    if (C % 8 != 0 || C < 8) return set_error(CL_ERR_UNSUPPORTED, c_msg);
     const int cpg = C / G;
     // channel ranges per image (whole groups, >= 128 channels = 256 contiguous bytes per row and a multiple of 8 channels)
     int cs = 1;
     while (G % (2 * cs) == 0 && (C / (2 * cs)) >= 128 && ((G / (2 * cs)) * cpg) % 8 == 0 && n * 16 * cs < 2 * num_sms()) cs *= 2;
     const int Cl = C / cs, Gl = G / cs;
-    if (Cl / 8 > GNC_THREADS) return 1;
+    if (Cl / 8 > GNC_THREADS) return set_error(CL_ERR_UNSUPPORTED, c_msg);
     const int chunks = Cl / 8;
     const int rows_par = GNC_THREADS / chunks;
-    const size_t smem = sizeof(double) * 2 * Gl + sizeof(float) * ((size_t)4 * Cl + (size_t)2 * rows_par * Cl);
-    if (smem > 100 * 1024 || (size_t)2 * rows_par * Cl * sizeof(float) < sizeof(double) * 2 * Gl) return 1;
-    static bool attr_done = false;
-    static int max_cluster = 8;
-    if (!attr_done) {
-        CL_CUDA_CHECK(cudaFuncSetAttribute(gn_cluster_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-        CL_CUDA_CHECK(cudaFuncSetAttribute(gn_cluster_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+    // [G][2] fp64 partial group sums, [4][C] fp32 coefficients, [2][rows_par][C] fp32 partial channel sums; the [G][2] fp64
+    // group totals reuse the last area after the exchange, so it is at least that large
+    const size_t part_bytes = sizeof(float) * 2 * rows_par * Cl, gsum_bytes = sizeof(double) * 2 * Gl;
+    const size_t smem = gsum_bytes + sizeof(float) * 4 * Cl + (part_bytes > gsum_bytes ? part_bytes : gsum_bytes);
+    static int max_cluster = 0, smem_max = 0;
+    static size_t smem_optin = 0;
+    if (max_cluster == 0) {
+        int dev = 0;
+        CL_CUDA_CHECK(cudaGetDevice(&dev));
+        CL_CUDA_CHECK(cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
         // clusters of 16 CTAs are "non-portable": opt in, and keep 8 when the device refuses
-        if (cudaFuncSetAttribute(gn_cluster_kernel<0>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess &&
-            cudaFuncSetAttribute(gn_cluster_kernel<1>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess)
-            max_cluster = 16;
+        max_cluster = cudaFuncSetAttribute(gn_cluster_kernel<BWD>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess ? 16 : 8;
         (void)cudaGetLastError();
-        attr_done = true;
     }
-    // CTAs per image: enough CTAs to fill the machine once, at least ~8 rows per row-slot, a power of two <= max_cluster
-    int cl = max_cluster;
+    if (smem > (size_t)smem_max)
+        return set_error(CL_ERR_UNSUPPORTED, "groupnorm: C = %d, G = %d needs %zu B of shared memory per CTA, the device allows %d", C, G,
+                         smem, smem_max);
+    if (smem > smem_optin) {           // 100 KiB (two CTAs per SM) covers every UNet / VAE / hint-encoder shape
+        const size_t optin = smem > 100 * 1024 ? smem : 100 * 1024;
+        CL_CUDA_CHECK(cudaFuncSetAttribute(gn_cluster_kernel<BWD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)optin));
+        smem_optin = optin;
+    }
+    // CTAs per image: enough CTAs to fill the machine once, at least ~8 rows per row-slot, a power of two <= max_cluster.
+    // Above 100 KiB only one CTA fits per SM, and a cluster of 16 would need 16 free SMs in one GPC: 8 at most then.
+    int cl = (smem > 100 * 1024 && max_cluster > 8) ? 8 : max_cluster;
     while (cl > 1 && (n * cl * cs > 3 * num_sms() || HW / cl < rows_par)) cl >>= 1;
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
@@ -792,20 +484,11 @@ static int gn_cluster_launch(const __nv_bfloat16* x, const __nv_bfloat16* dy, co
     cfg.blockDim = dim3(GNC_THREADS);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = stream;
-    cudaLaunchAttribute attr[2];
-    int na = 0;
-    if (cl > 1) {
-        attr[na].id = cudaLaunchAttributeClusterDimension;
-        attr[na].val.clusterDim.x = cl; attr[na].val.clusterDim.y = 1; attr[na].val.clusterDim.z = 1;
-        ++na;
-    }
-    if (pdl_enabled(CLB_FAMILY)) {
-        attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[na].val.programmaticStreamSerializationAllowed = 1;
-        ++na;
-    }
-    cfg.attrs = attr;
-    cfg.numAttrs = na;
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = cl; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+    cfg.attrs = &attr;
+    cfg.numAttrs = cl > 1 ? 1 : 0;
     const double inv_m = 1.0 / ((double)HW * (C / G));
     CL_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gn_cluster_kernel<BWD>, x, dy, gamma, beta, stats, out, dgamma, dbeta, HW, C, G, eps, inv_m,
                                      silu, accumulate));
@@ -813,82 +496,26 @@ static int gn_cluster_launch(const __nv_bfloat16* x, const __nv_bfloat16* dy, co
     return CL_OK;
 }
 
-extern "C" int64_t cl_groupnorm_ws_bytes(int n, int G, int C) { return (int64_t)16 * n * G + (int64_t)24 * n * C; }
-
-extern "C" int cl_groupnorm_fwd(const void* x, const float* gamma, const float* beta, void* y, float* stats,
-                                double* ws, int n, int HW, int C, int G, float eps, int silu, void* stream_) {
+extern "C" int cl_groupnorm_fwd(const void* x, const float* gamma, const float* beta, void* y, float* stats, int n, int HW, int C,
+                                int G, float eps, int silu, void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-    if (!x || !gamma || !beta || !y || !ws) return set_error(CL_ERR_INVALID, "cl_groupnorm_fwd: null pointer");
+    if (!x || !gamma || !beta || !y) return set_error(CL_ERR_INVALID, "cl_groupnorm_fwd: null pointer");
     if (stats == nullptr) return set_error(CL_ERR_INVALID, "cl_groupnorm_fwd: stats buffer is required");
     if (G <= 0 || C % G != 0) return set_error(CL_ERR_INVALID, "cl_groupnorm_fwd: C %% G != 0");
-    {
-        const int st = gn_cluster_launch<0>(reinterpret_cast<const __nv_bfloat16*>(x), nullptr, gamma, beta, stats,
-                                            reinterpret_cast<__nv_bfloat16*>(y), nullptr, nullptr, n, HW, C, G, eps, silu, 0, stream);
-        if (st <= 0) return st;          // launched (CL_OK) or failed; > 0: shape not covered -> three-kernel path below
-    }
-    int threads, rows_per_cta, grid_x;
-    CL_CHECK(gn_launch_geometry(HW, C, n, threads, rows_per_cta, grid_x));
-    double* gsum = ws;
-    float* coef = reinterpret_cast<float*>(ws + (size_t)2 * n * G);
-    CL_CUDA_CHECK(cudaMemsetAsync(gsum, 0, sizeof(double) * 2 * n * G, stream));
-    const size_t rsmem = (size_t)2 * (threads / (C / 8) + 1) * C * sizeof(float);
-    {
-        static bool done = false;
-        if (!done) {
-            CL_CUDA_CHECK(cudaFuncSetAttribute(gn_reduce_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-            done = true;
-        }
-    }
-    const __nv_bfloat16* xx = reinterpret_cast<const __nv_bfloat16*>(x);
-    launch_k(gn_reduce_kernel<0>, dim3(grid_x, n), threads, rsmem, stream, xx, nullptr, nullptr, nullptr, nullptr, gsum, nullptr, n,
-                                                                      HW, C, G, rows_per_cta, 0);
-    launch_k(gn_fwd_coef_kernel, n, 256, 0, stream, gsum, gamma, beta, stats, coef, n, C, G, 1.0 / ((double)HW * (C / G)), eps);
-    launch_k(gn_apply_kernel, dim3(gn_flat_blocks(HW, C, n, 2), n), 256, 0, stream, xx, coef, reinterpret_cast<__nv_bfloat16*>(y), n,
-                                                                              HW, C, silu);
-    count_launch(3);
-    CL_CUDA_CHECK(cudaGetLastError());
-    return CL_OK;
+    return gn_cluster_launch<0>(reinterpret_cast<const __nv_bfloat16*>(x), nullptr, gamma, beta, stats, reinterpret_cast<__nv_bfloat16*>(y),
+                                nullptr, nullptr, n, HW, C, G, eps, silu, 0, stream);
 }
 
-extern "C" int cl_groupnorm_bwd(const void* x, const void* dy, const float* gamma, const float* beta,
-                                const float* stats, void* dx, float* dgamma, float* dbeta, double* ws, int n, int HW,
-                                int C, int G, int silu, int accumulate, void* stream_) {
+extern "C" int cl_groupnorm_bwd(const void* x, const void* dy, const float* gamma, const float* beta, const float* stats, void* dx,
+                                float* dgamma, float* dbeta, int n, int HW, int C, int G, int silu, int accumulate, void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-    if (!x || !dy || !gamma || !beta || !stats || !dx || !ws) return set_error(CL_ERR_INVALID, "cl_groupnorm_bwd: null pointer");
+    if (!x || !dy || !gamma || !beta || !stats || !dx) return set_error(CL_ERR_INVALID, "cl_groupnorm_bwd: null pointer");
     if (G <= 0 || C % G != 0) return set_error(CL_ERR_INVALID, "cl_groupnorm_bwd: C %% G != 0");
     if (G > 4096) return set_error(CL_ERR_UNSUPPORTED, "cl_groupnorm_bwd: G <= 4096");
-    {
-        const int st = gn_cluster_launch<1>(reinterpret_cast<const __nv_bfloat16*>(x), reinterpret_cast<const __nv_bfloat16*>(dy), gamma,
-                                            beta, const_cast<float*>(stats), reinterpret_cast<__nv_bfloat16*>(dx), dgamma, dbeta, n, HW,
-                                            C, G, 0.f, silu, accumulate, stream);
-        if (st <= 0) return st;
-    }
-    int threads, rows_per_cta, grid_x;
-    CL_CHECK(gn_launch_geometry(HW, C, n, threads, rows_per_cta, grid_x));
-    float* coef = reinterpret_cast<float*>(ws + (size_t)2 * n * G);
-    float* csum = coef + (size_t)4 * n * C;
-    CL_CUDA_CHECK(cudaMemsetAsync(csum, 0, sizeof(float) * 2 * n * C, stream));
-    const size_t rsmem = (size_t)2 * (threads / (C / 8) + 1) * C * sizeof(float);
-    {
-        static bool done = false;
-        if (!done) {
-            CL_CUDA_CHECK(cudaFuncSetAttribute(gn_reduce_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-            done = true;
-        }
-    }
-    const __nv_bfloat16* xx = reinterpret_cast<const __nv_bfloat16*>(x);
-    const __nv_bfloat16* dd = reinterpret_cast<const __nv_bfloat16*>(dy);
-    launch_k(gn_reduce_kernel<1>, dim3(grid_x, n), threads, rsmem, stream, xx, dd, gamma, beta, stats, nullptr, csum, n, HW, C, G,
-                                                                      rows_per_cta, silu);
-    launch_k(gn_bwd_coef_kernel, n, 512, 2 * G * sizeof(float), stream, csum, gamma, beta, stats, coef, dgamma, dbeta, n, C, G,
-                                                                  1.f / ((float)HW * (C / G)));
-    launch_k(gn_bwd_apply_kernel, dim3(gn_flat_blocks(HW, C, n, 1), n), 256, 0, stream, xx, dd, coef, reinterpret_cast<__nv_bfloat16*>(dx),
-                                                                                  n, HW, C, silu, accumulate);
-    count_launch(3);
-    CL_CUDA_CHECK(cudaGetLastError());
-    return CL_OK;
+    return gn_cluster_launch<1>(reinterpret_cast<const __nv_bfloat16*>(x), reinterpret_cast<const __nv_bfloat16*>(dy), gamma, beta,
+                                const_cast<float*>(stats), reinterpret_cast<__nv_bfloat16*>(dx), dgamma, dbeta, n, HW, C, G, 0.f, silu,
+                                accumulate, stream);
 }
-
 extern "C" int cl_layernorm_fwd(const void* x, const float* gamma, const float* beta, void* y, float* stats, int T,
                                 int C, float eps, void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);

@@ -5,7 +5,6 @@
 #include <stdio.h>
 
 #include "common.cuh"
-#define CLB_FAMILY 128      // CLB_PDL_MASK bit of this file's kernels
 #include "host_common.h"
 #include "../../include/controllora_b200.h"
 

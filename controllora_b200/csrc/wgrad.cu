@@ -14,7 +14,6 @@
 
 #include "common.cuh"
 #include "wgmma.cuh"
-#define CLB_FAMILY 64      // CLB_PDL_MASK bit of this file's kernels
 #include "host_common.h"
 #include "../../include/controllora_b200.h"
 

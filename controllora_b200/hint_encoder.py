@@ -127,9 +127,8 @@ class HintEncoderEngine:
         return h
 
     # ------------------------------------------------------------------------------------------------ forward
-    def forward(self, ctx: Ctx, guide: torch.Tensor, on_level=None) -> List[Var]:
-        """guide: NCHW fp32 [B, 3, H, W] -> control states, one NHWC bf16 Var per level.  on_level(i) is called before level
-        i's ops are recorded (a tape entry recorded there runs AFTER level i's backward: the Trainer's gradient buckets)."""
+    def forward(self, ctx: Ctx, guide: torch.Tensor) -> List[Var]:
+        """guide: NCHW fp32 [B, 3, H, W] -> control states, one NHWC bf16 Var per level."""
         m = self.model
         ci = m.conv_in
         ops.conv_weight_prep(ci.weight, self.conv_in_w, None)
@@ -152,9 +151,7 @@ class HintEncoderEngine:
 
             ctx.tape.record(bwd_in)
         states = []
-        for i, (lvl_ops, pre_ops) in enumerate(self.levels):
-            if on_level is not None:
-                on_level(i)
+        for lvl_ops, pre_ops in self.levels:
             h = self._run_ops(ctx, h, lvl_ops)
             states.append(self._run_ops(ctx, h, pre_ops) if pre_ops else h)
         return states

@@ -26,7 +26,6 @@ from . import ops
 from .engine import Ctx, LoraSlot, Var
 
 BF16 = torch.bfloat16
-_FUSE_QKV = os.environ.get("CLB_FUSE_QKV", "1") != "0"
 
 
 def _is_v1(p) -> bool:
@@ -151,8 +150,8 @@ class LoraRuntime:
             kv_in = L.to_k.w.shape[1]
             lp.post_add = any(post_add)
             # V2 self-attention: k / v carry no LoRA (models.py:306-307) and read the same h' as q -> ONE fused q|k|v projection
-            # (N = 3C, the q adapter owns the first C output rows); CLB_FUSE_QKV=0 keeps three launches
-            lp.fuse_qkv = bool(_FUSE_QKV and _is_v2(p) and not L.is_cross and len(chain) == 1 and not any(post_add))
+            # (N = 3C, the q adapter owns the first C output rows)
+            lp.fuse_qkv = bool(_is_v2(p) and not L.is_cross and len(chain) == 1 and not any(post_add))
             lp.q = LoraSlot(3 * C if lp.fuse_qkv else C, C, dev)
             # post_add adapters read the projection's output: their `down` has C input features even for the text k / v
             lp.k = LoraSlot(C, C if lp.post_add else kv_in, dev)
@@ -491,7 +490,7 @@ class LoraRuntime:
         kvc = ctx.stash.get("kv_cache") if (ehs is not None and ctx.tape is None) else None
         if kvc is not None and L.name in kvc:
             k, v = kvc[L.name]                # text-state projections are timestep-invariant inside a denoise loop
-        elif _FUSE_QKV and ehs is not None and (lp.k is None or lp.k.rank == 0) and (lp.v is None or lp.v.rank == 0) and not kv_in.rg:
+        elif ehs is not None and (lp.k is None or lp.k.rank == 0) and (lp.v is None or lp.v.rank == 0) and not kv_in.rg:
             # no adapters on k / v (V2, or plain attention) and nothing to differentiate: k | v of the text states as ONE GEMM
             if getattr(L, "w_kv", None) is None:
                 L.w_kv = E.LinearW(torch.cat([L.to_k.w, L.to_v.w], 0).contiguous(), None, None)

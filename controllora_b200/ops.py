@@ -167,22 +167,6 @@ def _p(t):
     return C.c_void_p(0) if t is None else C.c_void_p(t.data_ptr())
 
 
-_ws_cache = {}
-
-
-def _gn_ws(device, n, G, Cc):
-    """GroupNorm scratch (cl_groupnorm_ws_bytes): fp64 group sums + per-(image, channel) coefficient / sum planes."""
-    nbytes = 16 * n * G + 24 * n * Cc
-    key = (device, "gn")
-    buf = _ws_cache.get(key)
-    if buf is None or buf.numel() * 8 < nbytes:
-        if buf is not None:
-            _WS_GRAVEYARD.append(buf)
-        buf = torch.empty((nbytes + 7) // 8 + 1024, device=device, dtype=torch.float64)
-        _ws_cache[key] = buf
-    return buf
-
-
 def attention_fwd(q, k, v, heads: int, scale: float, out=None, need_lse=True):
     """q [B, Nq, H*d], k/v [B, Nk, H*d] bf16 (last dim contiguous, arbitrary row stride) -> o [B, Nq, H*d], lse [B,H,Nq]."""
     from ._lib import AttnFwdArgs
@@ -216,8 +200,7 @@ def groupnorm_fwd(x, gamma, beta, G: int, eps: float, silu: bool, out=None):
     assert x.is_contiguous()
     y = torch.empty_like(x) if out is None else out
     stats = torch.empty(n, G, 2, device=x.device, dtype=torch.float32)
-    _call("cl_groupnorm_fwd", _p(x), _p(gamma), _p(beta), _p(y), _p(stats), _p(_gn_ws(x.device, n, G, C_)),
-          n, HW, C_, G, C.c_float(eps), int(silu))
+    _call("cl_groupnorm_fwd", _p(x), _p(gamma), _p(beta), _p(y), _p(stats), n, HW, C_, G, C.c_float(eps), int(silu))
     return y, stats
 
 
@@ -229,7 +212,7 @@ def groupnorm_bwd(x, dy, gamma, beta, stats, G: int, silu: bool, dx=None, accumu
         dx = torch.empty_like(x)
         accumulate = False
     _call("cl_groupnorm_bwd", _p(x), _p(dy), _p(gamma), _p(beta), _p(stats), _p(dx), _p(dgamma), _p(dbeta),
-          _p(_gn_ws(x.device, n, G, C_)), n, HW, C_, G, int(silu), int(accumulate))
+          n, HW, C_, G, int(silu), int(accumulate))
     return dx
 
 

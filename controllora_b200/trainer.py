@@ -92,23 +92,9 @@ class Trainer:
         self.gnorm_sq = torch.zeros(1, device=dev, dtype=torch.float32)
         self.step_idx = 0
         self.step_dev = torch.zeros(1, device=dev, dtype=torch.int64)     # device copy of step_idx (bias corrections inside the graph)
-        # data parallel: the gradient exchange is issued in THREE buckets on a side stream while the backward is still running
-        # (processor LoRAs once the UNet backward has finished, the deep hint-encoder levels once their backward has finished,
-        # the shallow levels at the end) - only the last, smallest bucket is exposed.  The arena order is the module order, so a
-        # bucket is one or two contiguous ranges of the flat gradient.
-        # CLB_DP_BUCKETS=1 opts in.  Default (what the 2-GPU runs validate): ONE all-reduce of the whole arena after the backward,
-        # outside the captured graph.  Round 2: the bucketed variant ran at 38.5 ms/step on 2 GPUs but its replicas drifted apart -
-        # bucket 0 was reduced while up to 15 LoRA dA / dB reductions were still sitting in the batched skinny queue (ops.SKINNY), so
-        # those gradients reached the arena AFTER the exchange.  _reduce_bucket now flushes the queue first; the world-2 gloo test
-        # (tests/test_dp_gloo.py, host-logic mode) checks bucketed == unbucketed == single-process big batch.  It stays opt-in until it
-        # has been re-measured on GPUs (the process also hung at teardown with NCCL inside the captured graph).
-        import os as _os
-        want_buckets = _os.environ.get("CLB_DP_BUCKETS", "0") == "1"
-        self._bucketed = bool(want_buckets and self.world > 1)   # False: ONE all-reduce after the backward (and outside a captured graph)
-        self._side = torch.cuda.Stream(device=dev) if (self._bucketed and dev.type == "cuda") else None
-        self._tail_in_graph = self.world == 1 or self._bucketed
-        self._reduced_in_step = False
-        self._buckets = self._make_buckets()
+        # data parallel: ONE all-reduce of the whole gradient arena after the backward.  With world > 1 it stays outside the
+        # captured graph (the graph holds forward + backward; the all-reduce and the optimizer launches follow each replay).
+        self._tail_in_graph = self.world == 1
         self.levels = None
         # CUDA-graph mode: the forward/backward (~1800 launches) is captured once and replayed, so the step costs the
         # host one graph launch instead of ~40 ms of Python/ctypes work and cannot become launch-bound.
@@ -142,8 +128,8 @@ class Trainer:
 
         With cuda_graph=True the first `graph_warmup` calls run eagerly, the next call captures the forward/backward
         into a CUDA graph (inputs are copied into static buffers first) and every later call replays it.  The graph holds
-        the WHOLE step: forward, backward, the bucketed gradient all-reduces (NCCL, on a side stream that forks from / joins the
-        capturing stream), clip + AdamW with a device-side step counter.  eager=True forces the uncaptured path."""
+        the forward and backward, and at world 1 also clip + AdamW with a device-side step counter; with world > 1 the gradient
+        all-reduce, clip and AdamW run after each replay.  eager=True forces the uncaptured path."""
         return self._run("noised", self._forward_backward, (noisy_latents, timesteps, ehs, guide, target), eager)
 
     def step_from_latents(self, latents: torch.Tensor, ehs: torch.Tensor, guide: torch.Tensor, eager: bool = False) -> torch.Tensor:
@@ -208,32 +194,22 @@ class Trainer:
             import sys
 
             n0 = _lib.launch_count()
-            while True:
-                graph = torch.cuda.CUDAGraph()
-                try:
-                    with torch.cuda.graph(graph, capture_error_mode="thread_local"):
-                        self._static_loss = fb(*self._static)
-                        if self._tail_in_graph:
-                            self._optimizer_tail()   # gradient exchange (side stream, world > 1), clip, AdamW: all inside the graph
-                    break
-                except Exception as ex:
-                    torch.cuda.synchronize()
-                    self._static_loss = None
-                    if self.world > 1 and self._bucketed:
-                        # NCCL refused to be captured: keep the graph for forward + backward, exchange gradients with one
-                        # all-reduce after the replay
-                        print(f"controllora_b200.Trainer: capturing the gradient all-reduce failed ({type(ex).__name__}: {ex}); "
-                              f"the collective and the optimizer stay outside the graph", file=sys.stderr, flush=True)
-                        self._bucketed, self._tail_in_graph, self._reduced_in_step = False, False, False
-                        n0 = _lib.launch_count()
-                        continue
-                    # capture is an optimisation of the launch path only: say so and keep training eagerly
-                    print(f"controllora_b200.Trainer: CUDA-graph capture failed ({type(ex).__name__}: {ex}); "
-                          f"continuing with per-kernel launches", file=sys.stderr, flush=True)
-                    self.cuda_graph = False
-                    loss = fb(*self._static)
-                    self._optimizer_tail()
-                    return loss
+            graph = torch.cuda.CUDAGraph()
+            try:
+                with torch.cuda.graph(graph, capture_error_mode="thread_local"):
+                    self._static_loss = fb(*self._static)
+                    if self._tail_in_graph:
+                        self._optimizer_tail()       # world 1: clip and AdamW inside the graph too
+            except Exception as ex:
+                torch.cuda.synchronize()
+                self._static_loss = None
+                # capture is an optimisation of the launch path only: say so and keep training eagerly
+                print(f"controllora_b200.Trainer: CUDA-graph capture failed ({type(ex).__name__}: {ex}); "
+                      f"continuing with per-kernel launches", file=sys.stderr, flush=True)
+                self.cuda_graph = False
+                loss = fb(*self._static)
+                self._optimizer_tail()
+                return loss
             self.launches_per_step = int(_lib.launch_count() - n0) + (0 if self._tail_in_graph else 3)
             self._graph = graph
             # capture executes nothing: the first replay below is this call's step
@@ -245,13 +221,7 @@ class Trainer:
     def _forward_backward(self, noisy_latents, timesteps, ehs, guide, target) -> torch.Tensor:
         tape = Tape()
         hctx = Ctx(tape=tape)
-        self._pending = [0, 1, 2] if self._bucketed else []
-        split = self._split_level
-
-        def on_level(i):
-            if i == split and self._bucketed:
-                tape.record(lambda: self._reduce_bucket(1))          # runs after the backward of levels >= split
-        states = [] if self.cl is None else self.hint.forward(hctx, guide, on_level=on_level)
+        states = [] if self.cl is None else self.hint.forward(hctx, guide)
         control = {}
         for procs, s in zip([] if self.cl is None else self.cl.lora_layers, states):
             n, H, W, C = s.data.shape
@@ -266,18 +236,10 @@ class Trainer:
                     c.grad = None
 
             tape.record(bridge)      # runs after every UNet backward op (incl. the per-level d-control GEMMs)
-        if self._bucketed:
-            tape.record(lambda: self._reduce_bucket(0))              # runs after every UNet backward op
         pred, ctx, rt = self.unet.run_engine(noisy_latents, timesteps, ehs, control, tape)
         loss, dpred = self._loss(pred.data, target)
         pred.grad = dpred
         tape.backward()
-        if self._bucketed:
-            for b in list(self._pending):
-                self._reduce_bucket(b)
-            if self._side is not None:
-                torch.cuda.current_stream().wait_stream(self._side)
-            self._reduced_in_step = True
         return loss
 
     def _loss(self, pred: torch.Tensor, target: torch.Tensor):
@@ -295,55 +257,11 @@ class Trainer:
         ops.axpy_matrix(prior.view(1, 1), loss.view(1, 1), self.prior_loss_weight)
         return loss, dpred
 
-    # ------------------------------------------------------------------------------------------------ gradient buckets
-    def _make_buckets(self):
-        """[[(lo, hi), ...] x 3]: 0 = everything whose gradient is complete when the UNet backward ends (lora_layers.* and
-        parameters that live in the UNet's processors), 1 = hint-encoder levels >= split, 2 = the rest (shallow levels, conv_in)."""
-        n_levels = len(getattr(self.cl, "down_blocks", [])) or 1
-        # level 0 (the 512x512 -> 64x64 pre-down path) is the longest part of the hint-encoder backward and runs last: everything
-        # above it is exchanged underneath it
-        self._split_level = 1 if n_levels > 1 else 0
-        groups = [[], [], []]
-        off = 0
-        for name, p in self._named_arena_params():
-            k = p.numel()
-            if name.startswith("lora_layers.") or name.startswith("extra."):
-                g = 0
-            else:
-                g = 2
-                parts = name.split(".")
-                if parts[0] in ("down_blocks", "pre_lora_layers") and len(parts) > 1 and parts[1].isdigit() and int(parts[1]) >= self._split_level:
-                    g = 1
-            r = groups[g]
-            if r and r[-1][1] == off:
-                r[-1] = (r[-1][0], off + k)
-            else:
-                r.append((off, off + k))
-            off += k
-        return groups
-
-    def _reduce_bucket(self, b: int) -> None:
-        """all-reduce(sum) of bucket b's gradient ranges on the side stream, ordered after everything the main stream has
-        launched so far; identical call order on every rank."""
-        if not self._bucketed or b not in self._pending:
-            return
-        self._pending.remove(b)
-        ops.SKINNY.flush()       # queued rank-r reductions (LoRA dA / dB) must be IN the arena before it is exchanged
-        if self._side is None:   # no side stream (host-logic tests on the CPU): same order, no overlap
-            for lo, hi in self._buckets[b]:
-                torch.distributed.all_reduce(self.flat_g[lo:hi], group=self.pg)
-            return
-        self._side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(self._side):
-            for lo, hi in self._buckets[b]:
-                torch.distributed.all_reduce(self.flat_g[lo:hi], group=self.pg)
-
     def _optimizer_tail(self) -> None:
-        """clip_grad_norm_ + AdamW + zero_grad (train_...:791-796) as three launches; the step count lives on the device, so the
-        tail can sit inside the captured graph."""
-        if not self._reduced_in_step:
-            self.arena.all_reduce()      # (no side stream: CPU arenas / world 1) one all-reduce(sum) over the whole gradient arena
-        self._reduced_in_step = False
+        """all-reduce(sum) of the gradient arena (nothing at world 1), then clip_grad_norm_ + AdamW + zero_grad
+        (train_...:791-796) as three launches; the step count lives on the device, so at world 1 the tail can sit inside the
+        captured graph."""
+        self.arena.all_reduce()
         ops.step_begin(self.gnorm_sq, self.step_dev)
         ops.sumsq(self.flat_g, self.gnorm_sq)
         # LambdaLR semantics: the k-th optimizer step (k = 1, 2, ...) runs with base_lr * lambda(k - 1)
@@ -361,8 +279,6 @@ class Trainer:
         like accelerate's 1/N loss scaling.  Not available on a Trainer that replays a captured step graph."""
         if self.cuda_graph:
             raise NotImplementedError("Trainer(cuda_graph=True) replays one captured whole step: gradient accumulation needs cuda_graph=False")
-        if self.world > 1 and self._bucketed:
-            raise NotImplementedError("gradient accumulation with the bucketed exchange (the buckets would be reduced once per micro-batch)")
         loss = self._forward_backward(noisy_latents, timesteps, ehs, guide, target)
         self._micro += 1
         return loss

@@ -136,14 +136,13 @@ int cl_attn_bwd(const cl_attn_bwd_args* args, void* stream);
  * K5: normalisation.  GroupNorm(+SiLU) on NHWC [n, HW, C] and LayerNorm on [T, C], forward and dX backward.
  * Replaces torch.nn.GroupNorm / F.silu / LayerNorm inside diffusers ResnetBlock2D, Transformer2DModel,
  * BasicTransformerBlock, UNet conv_norm_out, and models.py:515-543 (ConvBlock2D, where dgamma/dbeta are needed).
- * `ws` is caller-provided scratch of cl_groupnorm_ws_bytes(n, G, C) bytes (group sums, per-(image, channel) affine
- * coefficients, channel sums); `stats` (fp32 [n, G, 2] = mean, rstd) feeds the backward.
+ * GroupNorm is one kernel launch per direction and needs no scratch; `stats` (fp32 [n, G, 2] = mean, rstd) feeds the
+ * backward.
  * ---------------------------------------------------------------------------------------------------------- */
-int64_t cl_groupnorm_ws_bytes(int n, int G, int C);
-int cl_groupnorm_fwd(const void* x, const float* gamma, const float* beta, void* y, float* stats, double* ws,
+int cl_groupnorm_fwd(const void* x, const float* gamma, const float* beta, void* y, float* stats,
                      int n, int HW, int C, int G, float eps, int silu, void* stream);
 int cl_groupnorm_bwd(const void* x, const void* dy, const float* gamma, const float* beta, const float* stats,
-                     void* dx, float* dgamma /* nullable, accumulated */, float* dbeta, double* ws, int n, int HW,
+                     void* dx, float* dgamma /* nullable, accumulated */, float* dbeta, int n, int HW,
                      int C, int G, int silu, int accumulate_dx, void* stream);
 int cl_layernorm_fwd(const void* x, const float* gamma, const float* beta, void* y, float* stats /* [T,2] */,
                      int T, int C, float eps, void* stream);

@@ -24,11 +24,12 @@ def test_all_declared_symbols_are_exported(built_lib):
     assert not missing, f"declared in the header but not exported: {missing}"
 
 
-def test_version_and_error_string(built_lib):
+def test_abi_version_and_error_string(built_lib):
+    """ABI 101: the GroupNorm entry points take no scratch argument and cl_groupnorm_ws_bytes is gone."""
     from controllora_b200 import _lib
 
     lib = _lib.lib()
-    assert lib.cl_version() == 100
+    assert lib.cl_version() == 101
     assert isinstance(lib.cl_last_error(), bytes)
     assert _lib.launch_count() >= 0
 

@@ -63,15 +63,12 @@ def _worker(rank, world, port, q):
     full = _inputs(B)
     half = [v[rank * (B // world):(rank + 1) * (B // world)].to(dev) for v in full]
     tr._forward_backward(*half)
-    assert sum(hi - lo for b in tr._buckets for lo, hi in b) == tr.numel
-    if not tr._reduced_in_step:          # default: one all-reduce of the whole arena (CLB_DP_BUCKETS=1: issued in buckets already)
-        tr.arena.all_reduce()
+    tr.arena.all_reduce()                # one all-reduce of the whole arena
     torch.cuda.synchronize()
     g = (tr.flat_g[:tr.numel] * tr.arena.grad_scale).detach().cpu()
     # graph-replayed steps (forward + backward captured; all-reduce, clip, AdamW behind each replay) on rank-local data: the
     # replicas must stay bit-identical and the device step counter must follow the host's
     tr.flat_g.zero_()
-    tr._reduced_in_step = False
     tg = _build(dev)
     tg.cuda_graph, tg.graph_warmup = True, 2
     losses = []

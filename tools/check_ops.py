@@ -144,10 +144,13 @@ def groupnorm():
     import torch.nn.functional as F
     from controllora_b200 import ops
 
-    # incl. batch 8 (16-CTA clusters), HW not divisible by the cluster size (10x10), hint-encoder channel counts, 2x2 maps
+    # incl. batch 8 (16-CTA clusters), HW not divisible by the cluster size (10x10), hint-encoder channel counts, 2x2 maps, and
+    # wide shapes: group totals larger than the partial-sum area (C = G = 2056), more than 100 KiB of shared memory per CTA
+    # (8-CTA clusters), and the largest shared-memory footprint (C = G = 4096)
     for (n, H, C, G, silu, eps) in [(2, 64, 320, 32, True, 1e-5), (3, 16, 1280, 32, False, 1e-6), (2, 32, 2560, 32, True, 1e-5),
                                     (2, 64, 64, 32, True, 1e-6), (8, 32, 320, 32, True, 1e-5), (2, 10, 640, 32, True, 1e-5),
-                                    (1, 128, 32, 32, True, 1e-6), (3, 2, 128, 32, False, 1e-5), (16, 16, 1920, 32, True, 1e-5)]:
+                                    (1, 128, 32, 32, True, 1e-6), (3, 2, 128, 32, False, 1e-5), (16, 16, 1920, 32, True, 1e-5),
+                                    (1, 4, 2056, 2056, True, 1e-5), (17, 2, 4096, 512, False, 1e-5), (17, 4, 4096, 4096, True, 1e-6)]:
         x = (torch.randn(n, H, H, C, device="cuda") * 1.5 + 0.3).to(torch.bfloat16)
         g = 1 + 0.1 * torch.randn(C, device="cuda")
         b = 0.1 * torch.randn(C, device="cuda")
