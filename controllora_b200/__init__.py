@@ -8,8 +8,10 @@ from .models import (ControlLoRA, ControlLoRACrossAttnProcessor, ControlLoRACros
 from .unet_module import UNet2DConditionModel
 from .vae import AutoencoderKL
 from .clip import CLIPTextModel
+from .annotator import CannyDetector, canny_batch
 
 __all__ = [
     "ControlLoRA", "ControlLoRAOutput", "ControlLoRACrossAttnProcessor", "ControlLoRACrossAttnProcessorV2",
     "LoRACrossAttnProcessor", "LoRALinearLayer", "UNet2DConditionModel", "AutoencoderKL", "CLIPTextModel",
+    "CannyDetector", "canny_batch",
 ]

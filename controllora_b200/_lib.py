@@ -35,6 +35,9 @@ def lib() -> C.CDLL:
         _lib = C.CDLL(str(LIB_PATH))
         _lib.cl_last_error.restype = C.c_char_p
         _lib.cl_launch_count.restype = C.c_int64
+        _lib.cl_canny.restype = C.c_int
+        _lib.cl_canny.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                  C.c_void_p, C.c_void_p, C.c_void_p]
     return _lib
 
 

@@ -761,3 +761,32 @@ class SkinnyQueue:
 
 
 SKINNY = SkinnyQueue()
+
+
+def canny(images, thresholds, *, edges=None, guide=None, pixels=None):
+    """cv2.Canny per image (aperture 3, L2gradient=False, bit for bit) on a uint8 NHWC batch [B, H, W, C], C = 1 or 3.
+    thresholds: fp32 [B, 2] (lo, hi) on the device, read by the kernel (a captured graph replays with new values).  Fills
+    any of: edges uint8 [B, H, W] (0 / 255), guide fp32 [B, 3, H, W] (+-1), pixels fp32 [B, 3, H, W] = img / 127.5 - 1
+    (C = 3 only).  Returns (edges, guide, pixels)."""
+    _req(images, torch.uint8, "images")
+    _req(thresholds, torch.float32, "thresholds")
+    if images.dim() != 4 or not images.is_contiguous():
+        raise _lib.CLError(f"images: expected a contiguous [B, H, W, C] tensor, got shape {tuple(images.shape)}")
+    B, H, W, Cc = images.shape
+    if thresholds.shape != (B, 2) or not thresholds.is_contiguous():
+        raise _lib.CLError(f"thresholds: expected a contiguous [{B}, 2] tensor, got shape {tuple(thresholds.shape)}")
+    for name, t, dtype, shape in (("edges", edges, torch.uint8, (B, H, W)), ("guide", guide, torch.float32, (B, 3, H, W)),
+                                  ("pixels", pixels, torch.float32, (B, 3, H, W))):
+        if t is None:
+            continue
+        _req(t, dtype, name)
+        if tuple(t.shape) != shape or not t.is_contiguous():
+            raise _lib.CLError(f"{name}: expected a contiguous {shape} tensor, got shape {tuple(t.shape)}")
+        if t.device != images.device:
+            raise _lib.CLError(f"{name}: on {t.device}, images on {images.device}")
+    if thresholds.device != images.device:
+        raise _lib.CLError(f"thresholds: on {thresholds.device}, images on {images.device}")
+    labels = torch.empty(B * H * W, device=images.device, dtype=torch.int32)
+    check(_lib.lib().cl_canny(_ptr(images), B, H, W, Cc, _ptr(thresholds), _ptr(labels), _ptr(edges), _ptr(guide), _ptr(pixels),
+                              _stream()), "cl_canny")
+    return edges, guide, pixels

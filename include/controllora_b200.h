@@ -307,6 +307,24 @@ int cl_adamw_dev(float* p, float* g, float* m, float* v, int64_t n, float lr, fl
                  float weight_decay, const int64_t* step_dev, const float* gnorm_sq, float max_norm, float grad_scale,
                  int zero_grad, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Canny annotator: cv2.Canny(img, lo, hi) (aperture 3, L2gradient = false) bit for bit, and the float32 tensors the
+ * reference builds from it.  Replaces the OpenCV call and its arithmetic at process/diffusiondb_canny.py:35-45 (dataset of
+ * tasks/train_canny_v2.py: pixel_values = img / 127.5 - 1, guide = canny / 127.5 - 1 repeated to 3 channels),
+ * apps/gradio_canny2image.py:71-74 (apply_canny + HWC3 + [..., ::-1] / 127.5 - 1) and annotator/canny/__init__.py:6
+ * (CannyDetector, also used by tasks/make_dataset_diffusiondb_2m_first_5k_canny.py:27).
+ *   img:        uint8 NHWC [B, H, W, C], C = 1 or 3, channels used in the order given (a tie in gradient magnitude goes
+ *               to the first channel, so RGB and BGR input can differ); B*H*W < 2^31.
+ *   thresholds: device fp32 [B, 2] (lo, hi) per image, read on the device (swapped when lo > hi, then floored), so a
+ *               captured graph can replay with new values.
+ *   labels:     device int32 scratch [B*H*W].
+ *   outputs (any non-empty subset, NULL = skip): edges uint8 [B, H, W] (0 / 255); guide fp32 NCHW [B, 3, H, W] (+-1.0);
+ *               pixels fp32 NCHW [B, 3, H, W] = img / 127.5 - 1 with both operations rounded to fp32 (C = 3 only).
+ * Four launches whatever the data (union-find hysteresis), no host synchronisation.
+ * ---------------------------------------------------------------------------------------------------------- */
+int cl_canny(const uint8_t* img, int B, int H, int W, int C, const float* thresholds, int32_t* labels, uint8_t* edges,
+             float* guide, float* pixels, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
