@@ -6,7 +6,8 @@
 //
 // One CTA = one (batch, head, 128-query block), three warpgroups:
 //   warpgroup 0    TMA producer (one elected thread): Q once, then a two-stage mbarrier ring of K / V tiles of BN keys
-//                  (4-D tensor maps {d, H, N, B}; the head dim is padded to a multiple of 64 by TMA zero fill only)
+//                  (4-D tensor maps {d, H, N, B}; the head dim is padded to a multiple of 64 by TMA zero fill, and
+//                  S = Q K^T runs over ceil(d / 16) K16 steps only)
 //   warpgroups 1-2 64 query rows each: S = Q K^T with wgmma from shared memory, online softmax in the exp2 domain on the
 //                  accumulator registers (one row's statistics shared by the 4 lanes of a quad), O += P V with P as the
 //                  register A operand and V read MN-major, O kept in registers.
@@ -29,8 +30,9 @@ struct AttnFwdParams {
     int num_q_blocks;
 };
 
-template <int DCH>
+template <int D16>
 struct AttnFwdCfg {
+    static constexpr int DCH = head_chunks<D16>();
     static constexpr int BN = (DCH <= 2) ? 128 : 64;          // keys per stage (register budget of S + O)
     static constexpr int Q_BYTES = DCH * 128 * 128;
     static constexpr int KV_BYTES = DCH * BN * 128;
@@ -39,13 +41,13 @@ struct AttnFwdCfg {
     static constexpr int SMEM_BYTES = 1024 + Q_BYTES + STAGES * STAGE_BYTES + 256;
 };
 
-template <int DCH>
+template <int D16>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                       const __grid_constant__ CUtensorMap tmV, const AttnFwdParams p) {
     pdl_launch_dependents();
-    using Cfg = AttnFwdCfg<DCH>;
-    constexpr int BN = Cfg::BN;
+    using Cfg = AttnFwdCfg<D16>;
+    constexpr int BN = Cfg::BN, DCH = Cfg::DCH;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* sq = smem;
@@ -103,7 +105,7 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
         mbar_wait(&full_bar[stage], phase);
         const uint32_t k_addr = smem_u32(skv + stage * Cfg::STAGE_BYTES), v_addr = k_addr + Cfg::KV_BYTES;
         float s[BN / 2];
-        att_abt<DCH, 128, BN>(s, q_addr, row0, k_addr);
+        att_abt<D16, 128, BN>(s, q_addr, row0, k_addr);
         // scaled scores in the log2 domain, keys beyond Nk masked; s[nt*4 + c]: row lane/4 + 8(c/2), key 8nt + 2(lane%4) + c%2
         float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
@@ -141,7 +143,7 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
                 o[c][jj * 4] *= corr[0]; o[c][jj * 4 + 1] *= corr[0];
                 o[c][jj * 4 + 2] *= corr[1]; o[c][jj * 4 + 3] *= corr[1];
             }
-        att_pv<DCH, BN, BN / 16>(o, pa, v_addr, 0, DCH);
+        att_pv<DCH, 64, BN, BN / 16>(o, pa, v_addr, 0);
         if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[stage]);
         if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
     }
@@ -165,9 +167,9 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
     store_rows<DCH>(o, 1.f, p.o + (long long)b * p.Nq * p.ldo + h * p.d, p.ldo, q0 + row0, p.Nq, p.d, 0, lane, w4);
 }
 
-template <int DCH>
+template <int D16>
 static int launch_attn_fwd(const cl_attn_fwd_args* a, cudaStream_t stream) {
-    using Cfg = AttnFwdCfg<DCH>;
+    using Cfg = AttnFwdCfg<D16>;
     CUtensorMap tq, tk, tv;
     CL_CHECK(make_head_map(&tq, a->q, a->B, a->H, a->Nq, a->d, a->ldq, 128));
     CL_CHECK(make_head_map(&tk, a->k, a->B, a->H, a->Nk, a->d, a->ldk, Cfg::BN));
@@ -179,12 +181,12 @@ static int launch_attn_fwd(const cl_attn_fwd_args* a, cudaStream_t stream) {
     p.num_q_blocks = (a->Nq + 127) / 128;
     static bool attr_done = false;
     if (!attr_done) {
-        CL_CUDA_CHECK(cudaFuncSetAttribute(attn_fwd_wgmma_kernel<DCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+        CL_CUDA_CHECK(cudaFuncSetAttribute(attn_fwd_wgmma_kernel<D16>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
         attr_done = true;
     }
     const long long grid = (long long)a->B * a->H * p.num_q_blocks;
     if (grid > 0x7fffffffLL) return set_error(CL_ERR_UNSUPPORTED, "cl_attn_fwd: too many blocks");
-    launch_k(attn_fwd_wgmma_kernel<DCH>, (unsigned)grid, ATT_THREADS, Cfg::SMEM_BYTES, stream, tq, tk, tv, p);
+    launch_k(attn_fwd_wgmma_kernel<D16>, (unsigned)grid, ATT_THREADS, Cfg::SMEM_BYTES, stream, tq, tk, tv, p);
     count_launch();
     CL_CUDA_CHECK(cudaGetLastError());
     return CL_OK;
@@ -200,7 +202,5 @@ extern "C" int cl_attn_fwd(const cl_attn_fwd_args* a, void* stream_) {
     if (a->d % 8 != 0 || a->d <= 0 || a->d > 192) return set_error(CL_ERR_UNSUPPORTED, "cl_attn_fwd: head dim must be a multiple of 8, <= 192");
     if ((a->ldq % 8) || (a->ldk % 8) || (a->ldv % 8) || (a->ldo % 8)) return set_error(CL_ERR_INVALID, "cl_attn_fwd: row strides must be multiples of 8");
     if (a->B <= 0 || a->H <= 0 || a->Nq <= 0 || a->Nk <= 0) return set_error(CL_ERR_INVALID, "cl_attn_fwd: dims");
-    if (a->d <= 64) return launch_attn_fwd<1>(a, stream);
-    if (a->d <= 128) return launch_attn_fwd<2>(a, stream);
-    return launch_attn_fwd<3>(a, stream);
+    return with_head_d16(a->d, [&](auto d16) { return launch_attn_fwd<decltype(d16)::value>(a, stream); });
 }
