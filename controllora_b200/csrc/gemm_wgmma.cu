@@ -2,11 +2,15 @@
 //
 //   D[M,N] = epilogue( A[M,K] * B[N,K]^T ),  bf16 operands, fp32 accumulation in registers.
 //
-// One CTA per 128 x BN output tile (x one K range under split-K), three warpgroups:
-//   warpgroup 0    TMA producer (one elected thread of warp 0): A tile 128 x BK, B tile BN x BK [+16 LoRA-down rows],
-//                  128B (BK = 64) or 64B (BK = 32) swizzle, mbarrier ring of up to 8 stages
-//   warpgroups 1-2 consumers: rows 0-63 / 64-127 of the tile, wgmma.m64n(BN+EXT)k16 straight from the swizzled stages,
+// One CTA per 128 x BN output tile (x one K range under split-K), 288 threads:
+//   warpgroups 0-1 consumers: rows 0-63 / 64-127 of the tile, wgmma.m64n(BN+EXT)k16 straight from the swizzled stages,
 //                  then the epilogue from the accumulator registers (bias, per-image row bias, residual, LoRA, store).
+//   warp 8         TMA producer (one elected thread): A tile 128 x BK, B tile BN x BK [+16 LoRA-down rows],
+//                  128B (BK = 64) or 64B (BK = 32) swizzle, mbarrier ring of up to 8 stages
+// Occupancy OCC = 1 or 2 CTAs per SM is a template parameter: it sets the register cap (224 or 96 per thread; no
+// setmaxnreg, so the producer warp holds as many as a consumer) and the shared memory a launch may use.  With two CTAs on
+// an SM, one CTA's prologue, pipeline fill and register epilogue run while the other's MMAs do, which is what short-K
+// tiles (a few k-blocks each) need; deep-K tiles keep one CTA per SM and the deeper ring.
 // LoRA (EXT = 16): the 16 extra B rows (bf16 hi / lo halves of the rank-r down matrix) make the main loop produce
 // t = x A^T in 16 extra accumulator columns; the epilogue forms t (+ t_add, -> t_out) and adds scale * t B_up^T in fp32.
 // The A operand is either a plain row-major matrix or an NHWC image read as 3x3 windows (implicit GEMM: the
@@ -26,8 +30,17 @@
 namespace clb {
 
 static constexpr int BLOCK_M = 128;
-static constexpr int NUM_THREADS = 384;
-static constexpr int SMEM_LIMIT = 232448;     // 227 KB of dynamic shared memory per block
+static constexpr int NUM_THREADS = 288;
+static constexpr int PRODUCER_WARP = 8;
+// Dynamic shared memory per CTA: 227 KB for one CTA per SM; for two, half of the SM's 228 KB less the 1 KB the hardware
+// reserves per CTA.
+template <int OCC> struct GemmOcc {
+    static_assert(OCC == 1 || OCC == 2, "OCC");
+    static constexpr int SMEM_LIMIT = OCC == 1 ? 232448 : 115712;
+    // One CTA: 65536 registers / 288 threads, rounded down to 8.  Two CTAs: 18 warps over the SM's four 16384-register
+    // quarters put 5 warps on one quarter, so 16384 / (5 * 32) = 102, rounded down to 8.
+    static constexpr int MAX_REGS = OCC == 1 ? 224 : 96;
+};
 
 struct GemmParams {
     int M, N, K;
@@ -95,8 +108,8 @@ __device__ __forceinline__ void decode_row(const GemmParams& p, int m_blk, int r
     }
 }
 
-template <int BN, int EXT, int BK>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
+template <int BN, int EXT, int BK, int OCC>
+__global__ void __maxnreg__(GemmOcc<OCC>::MAX_REGS)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmE, const GemmParams p, const int num_stages) {
     pdl_launch_dependents();
@@ -117,7 +130,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const int kb0 = split * p.kb_per_split;
     const int kb1 = min(p.num_k_blocks, kb0 + p.kb_per_split);
 
-    if (warp_idx == 0 && lane == 0) {
+    if (warp_idx == PRODUCER_WARP && lane == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
         if (EXT) tma_prefetch_desc(&tmE);
@@ -130,9 +143,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     __syncthreads();
     pdl_wait();   // everything above touched only shared memory and kernel parameters
 
-    if (wg == 0) {
-        setmaxnreg_dec<40>();
-        if (warp_idx == 0 && elect_one_sync()) {
+    if (warp_idx == PRODUCER_WARP) {
+        if (elect_one_sync()) {
             int tw = 0, th = 0, tn = 0;
             if (p.a_mode != 0) {
                 tw = m_blk % p.tiles_w;
@@ -169,12 +181,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         return;
     }
 
-    setmaxnreg_inc<232>();
     // ===================================================== consumers: main loop
     float acc[Cfg::ACC];
 #pragma unroll
     for (int i = 0; i < Cfg::ACC; ++i) acc[i] = 0.f;
-    const uint32_t a_off = uint32_t(wg - 1) * 64 * Cfg::ROW_BYTES;
+    const uint32_t a_off = uint32_t(wg) * 64 * Cfg::ROW_BYTES;
     {
         int stage = 0, prev = -1;
         uint32_t phase = 0;
@@ -200,68 +211,78 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     // ===================================================== epilogue from registers
     // accumulator layout of wgmma m64nNk16: acc[j*4 + i*2 + c] = D[row w*16 + lane/4 + 8i][col 8j + 2*(lane%4) + c]
     const int w4 = warp_idx & 3, q = lane & 3;
+    // Both rows of this lane first (row index, row_bias group, LoRA t), then the columns: each column's lora_up values are
+    // loaded once for the two rows.
+    int m[2], grp[2];
+    float t[2][8];
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
-        const int r = (wg - 1) * 64 + w4 * 16 + (lane >> 2) + 8 * i;
-        int m, grp;
-        decode_row(p, m_blk, r, m, grp);
-        float t[8];
+        decode_row(p, m_blk, wg * 64 + w4 * 16 + (lane >> 2) + 8 * i, m[i], grp[i]);
         if (EXT) {
             // t[j] = e[j] + e[j + 8]: this lane holds columns 2q, 2q+1 of both halves; gather the quad's 8 values
             const float t0 = acc[(BN / 8) * 4 + i * 2] + acc[(BN / 8 + 1) * 4 + i * 2];
             const float t1 = acc[(BN / 8) * 4 + i * 2 + 1] + acc[(BN / 8 + 1) * 4 + i * 2 + 1];
 #pragma unroll
             for (int qq = 0; qq < 4; ++qq) {
-                t[2 * qq] = __shfl_sync(0xffffffffu, t0, (lane & ~3) | qq);
-                t[2 * qq + 1] = __shfl_sync(0xffffffffu, t1, (lane & ~3) | qq);
+                t[i][2 * qq] = __shfl_sync(0xffffffffu, t0, (lane & ~3) | qq);
+                t[i][2 * qq + 1] = __shfl_sync(0xffffffffu, t1, (lane & ~3) | qq);
             }
             const int rp = p.lora_rp;
-            if (m >= 0) {
+            if (m[i] >= 0) {
+                const long long tb = (long long)m[i] * rp;
+                float o0 = t0, o1 = t1;   // this lane's own columns 2q, 2q+1, so t is never indexed by the lane
                 if (p.t_add != nullptr) {
+                    if (2 * q < rp) { o0 += p.t_add[tb + 2 * q]; o1 += p.t_add[tb + 2 * q + 1]; }   // rp is even
 #pragma unroll
-                    for (int j = 0; j < 8; ++j)
-                        if (j < rp) t[j] += p.t_add[(long long)m * rp + j];
+                    for (int jj = 0; jj < 8; ++jj)
+                        if (jj < rp) t[i][jj] += p.t_add[tb + jj];
                 }
-                if (p.t_out != nullptr && n_blk == 0) {
-#pragma unroll
-                    for (int c = 0; c < 2; ++c)
-                        if (2 * q + c < rp) p.t_out[(long long)m * rp + 2 * q + c] = t[2 * q + c];
-                }
+                if (p.t_out != nullptr && n_blk == 0 && 2 * q < rp) { p.t_out[tb + 2 * q] = o0; p.t_out[tb + 2 * q + 1] = o1; }
             }
 #pragma unroll
-            for (int j = 0; j < 8; ++j) t[j] = (j < rp) ? t[j] * p.lora_scale : 0.f;
+            for (int jj = 0; jj < 8; ++jj) t[i][jj] = (jj < rp) ? t[i][jj] * p.lora_scale : 0.f;
         }
-        if (m < 0) continue;
+    }
 #pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-            const int n = n_blk * BN + 8 * j + 2 * q;
-            if (n >= p.N) continue;          // N % 4 == 0: n < N implies n + 1 < N
+    for (int j = 0; j < BN / 8; ++j) {
+        const int n = n_blk * BN + 8 * j + 2 * q;
+        if (n >= p.N) continue;          // N % 4 == 0: n < N implies n + 1 < N
+        float u0[8], u1[8];
+        if (EXT) {
+            const float* up = p.lora_up + (long long)n * p.lora_rp;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+                u0[jj] = jj < p.lora_rp ? __ldg(up + jj) : 0.f;
+                u1[jj] = jj < p.lora_rp ? __ldg(up + p.lora_rp + jj) : 0.f;
+            }
+        }
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            if (m[i] < 0) continue;
             float v0 = acc[j * 4 + i * 2], v1 = acc[j * 4 + i * 2 + 1];
             if (EXT) {
-                const float* u0 = p.lora_up + (long long)n * p.lora_rp;
-                const float* u1 = u0 + p.lora_rp;
 #pragma unroll
                 for (int jj = 0; jj < 8; ++jj) {
-                    if (jj < p.lora_rp) { v0 = fmaf(t[jj], __ldg(u0 + jj), v0); v1 = fmaf(t[jj], __ldg(u1 + jj), v1); }
+                    if (jj < p.lora_rp) { v0 = fmaf(t[i][jj], u0[jj], v0); v1 = fmaf(t[i][jj], u1[jj], v1); }
                 }
             }
             if (p.splits > 1) {     // host cleared bias / row_bias / residual: the finishing kernel applies them
-                *reinterpret_cast<float2*>(p.split_ws + (long long)split * p.M * p.N + (long long)m * p.N + n) = make_float2(v0, v1);
+                *reinterpret_cast<float2*>(p.split_ws + (long long)split * p.M * p.N + (long long)m[i] * p.N + n) = make_float2(v0, v1);
                 continue;
             }
             if (p.bias != nullptr) { v0 += __ldg(p.bias + n); v1 += __ldg(p.bias + n + 1); }
             if (p.row_bias != nullptr) {
-                const float2 rb = *reinterpret_cast<const float2*>(p.row_bias + (long long)grp * p.ld_rb + n);
+                const float2 rb = *reinterpret_cast<const float2*>(p.row_bias + (long long)grp[i] * p.ld_rb + n);
                 v0 += rb.x; v1 += rb.y;
             }
             if (p.residual != nullptr) {
-                const float2 rr = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(p.residual + (long long)m * p.ldr + n));
+                const float2 rr = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(p.residual + (long long)m[i] * p.ldr + n));
                 v0 += rr.x; v1 += rr.y;
             }
             if (p.out_fp32) {
-                *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + (long long)m * p.ldd + n) = make_float2(v0, v1);
+                *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + (long long)m[i] * p.ldd + n) = make_float2(v0, v1);
             } else {
-                *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out) + (long long)m * p.ldd + n) = pack_bf16x2(v0, v1);
+                *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out) + (long long)m[i] * p.ldd + n) = pack_bf16x2(v0, v1);
             }
         }
     }
@@ -314,10 +335,13 @@ splitk_finish_kernel(const float* __restrict__ ws, int splits, int M, int N, con
 // host side
 // =====================================================================================================
 
-template <int BN, int EXT, int BK = 64>
+// Launches the GEMM; with `resident` set, launches nothing and stores how many CTAs of this instantiation the device keeps
+// resident per SM at the shared-memory size the launch would use.
+template <int BN, int EXT, int BK, int OCC>
 static int launch_gemm(const CUtensorMap& tA, const CUtensorMap& tB, const CUtensorMap& tE, const GemmParams& p_in,
-                       cudaStream_t stream) {
+                       cudaStream_t stream, int* resident) {
     using Cfg = GemmCfg<BN, EXT, BK>;
+    constexpr int SMEM_LIMIT = GemmOcc<OCC>::SMEM_LIMIT;
     GemmParams p = p_in;
     const int fixed = 1024 /*align slack*/ + 256 /*barriers*/;
     int stages = (SMEM_LIMIT - fixed) / Cfg::STAGE_BYTES;
@@ -330,10 +354,14 @@ static int launch_gemm(const CUtensorMap& tA, const CUtensorMap& tB, const CUten
     if (p.splits > 1) { p.bias = nullptr; p.row_bias = nullptr; p.residual = nullptr; }
     static bool attr_done = false;
     if (!attr_done) {
-        CL_CUDA_CHECK(cudaFuncSetAttribute(gemm_wgmma_kernel<BN, EXT, BK>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
+        CL_CUDA_CHECK(cudaFuncSetAttribute(gemm_wgmma_kernel<BN, EXT, BK, OCC>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
         attr_done = true;
     }
-    launch_k_pdl(gemm_wgmma_kernel<BN, EXT, BK>, (unsigned)grid, NUM_THREADS, smem_bytes, stream, tA, tB, tE, p, stages);
+    if (resident != nullptr) {
+        CL_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(resident, gemm_wgmma_kernel<BN, EXT, BK, OCC>, NUM_THREADS, smem_bytes));
+        return CL_OK;
+    }
+    launch_k_pdl(gemm_wgmma_kernel<BN, EXT, BK, OCC>, (unsigned)grid, NUM_THREADS, smem_bytes, stream, tA, tB, tE, p, stages);
     count_launch();
     if (p.splits > 1) {
         const long long quads = (long long)p.M * (p.N / 4);
@@ -350,20 +378,23 @@ static int launch_gemm(const CUtensorMap& tA, const CUtensorMap& tB, const CUten
 
 using namespace clb;
 
-// Output-tile plan: block_n and the number of K splits.  Cost model: a CTA streams (128 + bn) operand rows per k-block
+// Output-tile plan: block_n, the number of K splits and CTAs per SM (rule at the end of plan_tiles).  Cost model: a CTA streams (128 + bn) operand rows per k-block
 // and the kernel runs `waves` rounds of tiles, so
 //   cost = waves(tiles * splits) * (128 + bn + 32) * ceil(nkb / splits)          (+32: per-tile epilogue / ramp)
 // Splitting K is only considered when the (m, n) tiles leave more than half of the SMs idle and every split keeps
 // >= 8 k-blocks.  The caller provides split_ws = splits * M * N floats (cl_gemm_split_hint tells how many).
-struct TilePlan { int bn, splits; };
+struct TilePlan { int bn, splits, occ; };
 
 static inline int gemm_block_k(const cl_gemm_args* a) { return (a->a_mode != 0 && a->C % 64 != 0) ? 32 : 64; }
+
+// The instantiations that compile within GemmOcc<2>::MAX_REGS registers without spilling.
+static inline bool gemm_fits_two_ctas(int bn, bool lora, int BK) { return !lora && (BK == 32 ? bn <= 128 : bn == 128); }
 
 static TilePlan plan_tiles(const cl_gemm_args* a, int BK, int num_m_blocks, bool allow_split) {
     const bool lora = a->lora_up != nullptr;
     const int nkb = (a->K + BK - 1) / BK;
     const int sms = num_sms();
-    TilePlan best = {0, 1};
+    TilePlan best = {0, 1, 1};
     long long best_cost = -1;
     static const int cands[5] = {256, 160, 128, 64, 32};
     for (int ci = 0; ci < 5; ++ci) {
@@ -384,7 +415,7 @@ static TilePlan plan_tiles(const cl_gemm_args* a, int BK, int num_m_blocks, bool
         splits = (nkb + kbps - 1) / kbps;
         const long long waves = ((long long)tiles * splits + sms - 1) / sms;
         const long long cost = waves * (128 + bn + 32) * kbps;
-        if (best_cost < 0 || cost < best_cost) { best_cost = cost; best = {bn, splits}; }
+        if (best_cost < 0 || cost < best_cost) { best_cost = cost; best = {bn, splits, 1}; }
     }
     if (best_cost < 0) {   // no candidate divides N: tail tiles
         if (lora) best.bn = (a->N % 128 == 0) ? 128 : 160;
@@ -393,6 +424,14 @@ static TilePlan plan_tiles(const cl_gemm_args* a, int BK, int num_m_blocks, bool
         else if (a->N <= 128 || BK == 32) best.bn = 128;
         else best.bn = 160;
         best.splits = 1;
+    }
+    // Two CTAs per SM for unsplit short-K launches (<= 20 k-blocks per tile) whose tiles fill every one of the 2 * sms
+    // CTA slots: then one CTA's prologue, pipeline fill and epilogue overlap the other's MMAs.  Measured on the bench step
+    // (H100 SXM): the 9-18 k-block launches with >= 1024 tiles ran 0.79-0.85x the one-CTA time at BK 64 and BN 128;
+    // launches of 80-240 tiles were slower at two CTAs per SM (pairs share SMs while others idle), deep-K ones were too.
+    if (best.splits == 1 && nkb <= 20 && gemm_fits_two_ctas(best.bn, lora, BK)) {
+        const long long tiles = (long long)num_m_blocks * ((a->N + best.bn - 1) / best.bn);
+        if (tiles >= 2LL * sms) best.occ = 2;
     }
     return best;
 }
@@ -403,8 +442,36 @@ extern "C" int cl_gemm_split_hint(const cl_gemm_args* a) {
     return plan_tiles(a, gemm_block_k(a), (a->M + BLOCK_M - 1) / BLOCK_M, true).splits;
 }
 
-extern "C" int cl_gemm(const cl_gemm_args* a, void* stream_) {
-    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+static int dispatch_gemm(const CUtensorMap& tA, const CUtensorMap& tB, const CUtensorMap& tE, const GemmParams& p,
+                         cudaStream_t stream, int* q, int bn_sel, bool two, bool lora, int BK) {
+    if (BK == 32) {
+        if (lora) return set_error(CL_ERR_UNSUPPORTED, "cl_gemm: LoRA epilogue is not instantiated for 32-channel convs");
+        switch (bn_sel) {
+            case 32: return two ? launch_gemm<32, 0, 32, 2>(tA, tB, tE, p, stream, q) : launch_gemm<32, 0, 32, 1>(tA, tB, tE, p, stream, q);
+            case 64: return two ? launch_gemm<64, 0, 32, 2>(tA, tB, tE, p, stream, q) : launch_gemm<64, 0, 32, 1>(tA, tB, tE, p, stream, q);
+            case 128: return two ? launch_gemm<128, 0, 32, 2>(tA, tB, tE, p, stream, q) : launch_gemm<128, 0, 32, 1>(tA, tB, tE, p, stream, q);
+            default: return set_error(CL_ERR_UNSUPPORTED, "cl_gemm: block_n for 32-channel convs must be 32/64/128");
+        }
+    }
+    if (lora) {
+        switch (bn_sel) {
+            case 64: return launch_gemm<64, 16, 64, 1>(tA, tB, tE, p, stream, q);
+            case 128: return launch_gemm<128, 16, 64, 1>(tA, tB, tE, p, stream, q);
+            case 160: return launch_gemm<160, 16, 64, 1>(tA, tB, tE, p, stream, q);
+            default: return set_error(CL_ERR_UNSUPPORTED, "cl_gemm: block_n for LoRA must be 64/128/160");
+        }
+    }
+    switch (bn_sel) {
+        case 64: return launch_gemm<64, 0, 64, 1>(tA, tB, tE, p, stream, q);
+        case 128: return two ? launch_gemm<128, 0, 64, 2>(tA, tB, tE, p, stream, q) : launch_gemm<128, 0, 64, 1>(tA, tB, tE, p, stream, q);
+        case 160: return launch_gemm<160, 0, 64, 1>(tA, tB, tE, p, stream, q);
+        case 256: return launch_gemm<256, 0, 64, 1>(tA, tB, tE, p, stream, q);
+        default: return set_error(CL_ERR_UNSUPPORTED, "cl_gemm: block_n must be 64/128/160/256");
+    }
+}
+
+// cl_gemm, or with `info` set, cl_gemm_plan: info = {block_n, splits, ctas_per_sm, resident_per_sm} and no launch.
+static int run_gemm(const cl_gemm_args* a, cudaStream_t stream, int32_t* info) {
     if (a == nullptr || a->a == nullptr || a->b == nullptr || a->out == nullptr)
         return set_error(CL_ERR_INVALID, "cl_gemm: null pointer");
     if (a->M <= 0 || a->N <= 0 || a->K <= 0) return set_error(CL_ERR_INVALID, "cl_gemm: non-positive dims");
@@ -473,8 +540,8 @@ extern "C" int cl_gemm(const cl_gemm_args* a, void* stream_) {
     const int bn_sel = plan.bn;
     {
         static const int dbg = [] { const char* e = getenv("CLB_GEMM_DEBUG"); return (e && e[0] == '1') ? 1 : 0; }();
-        if (dbg) fprintf(stderr, "cl_gemm M=%d N=%d K=%d mode=%d lora=%d -> bn=%d splits=%d (asked bn=%d split_k=%d)\n", a->M, a->N, a->K,
-                         a->a_mode, lora ? 1 : 0, bn_sel, plan.splits, a->block_n, a->split_k);
+        if (dbg) fprintf(stderr, "cl_gemm M=%d N=%d K=%d mode=%d lora=%d -> bn=%d splits=%d occ=%d (asked bn=%d split_k=%d)\n", a->M, a->N,
+                         a->K, a->a_mode, lora ? 1 : 0, bn_sel, plan.splits, plan.occ, a->block_n, a->split_k);
     }
     p.num_n_blocks = (a->N + bn_sel - 1) / bn_sel;
     p.splits = 1;
@@ -509,28 +576,17 @@ extern "C" int cl_gemm(const cl_gemm_args* a, void* stream_) {
     if (p.row_bias && p.rows_per_group <= 0) return set_error(CL_ERR_INVALID, "cl_gemm: rows_per_group");
     if ((p.ldd % 4) || (p.residual && (p.ldr % 4))) return set_error(CL_ERR_INVALID, "cl_gemm: ldd/ldr % 4");
 
-    if (BK == 32) {
-        if (lora) return set_error(CL_ERR_UNSUPPORTED, "cl_gemm: LoRA epilogue is not instantiated for 32-channel convs");
-        switch (bn_sel) {
-            case 32: return launch_gemm<32, 0, 32>(tA, tB, tE, p, stream);
-            case 64: return launch_gemm<64, 0, 32>(tA, tB, tE, p, stream);
-            case 128: return launch_gemm<128, 0, 32>(tA, tB, tE, p, stream);
-            default: return set_error(CL_ERR_UNSUPPORTED, "cl_gemm: block_n for 32-channel convs must be 32/64/128");
-        }
-    }
-    if (lora) {
-        switch (bn_sel) {
-            case 64: return launch_gemm<64, 16>(tA, tB, tE, p, stream);
-            case 128: return launch_gemm<128, 16>(tA, tB, tE, p, stream);
-            case 160: return launch_gemm<160, 16>(tA, tB, tE, p, stream);
-            default: return set_error(CL_ERR_UNSUPPORTED, "cl_gemm: block_n for LoRA must be 64/128/160");
-        }
-    }
-    switch (bn_sel) {
-        case 64: return launch_gemm<64, 0>(tA, tB, tE, p, stream);
-        case 128: return launch_gemm<128, 0>(tA, tB, tE, p, stream);
-        case 160: return launch_gemm<160, 0>(tA, tB, tE, p, stream);
-        case 256: return launch_gemm<256, 0>(tA, tB, tE, p, stream);
-        default: return set_error(CL_ERR_UNSUPPORTED, "cl_gemm: block_n must be 64/128/160/256");
-    }
+    const bool two = plan.occ == 2;
+    int resident = 0;
+    int* const q = info != nullptr ? &resident : nullptr;
+    const int st = dispatch_gemm(tA, tB, tE, p, stream, q, bn_sel, two, lora, BK);
+    if (info != nullptr && st == CL_OK) { info[0] = bn_sel; info[1] = p.splits; info[2] = plan.occ; info[3] = resident; }
+    return st;
+}
+
+extern "C" int cl_gemm(const cl_gemm_args* a, void* stream) { return run_gemm(a, reinterpret_cast<cudaStream_t>(stream), nullptr); }
+
+extern "C" int cl_gemm_plan(const cl_gemm_args* a, int32_t* info) {
+    if (info == nullptr) return set_error(CL_ERR_INVALID, "cl_gemm_plan: null info");
+    return run_gemm(a, nullptr, info);
 }

@@ -26,9 +26,11 @@ static inline void launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, siz
 
 // As launch_k, with the programmatic-stream-serialization attribute: inside a stream (or a captured CUDA graph) the grid
 // may start while the previous kernel drains; every kernel of this library executes griddepcontrol.wait (pdl_wait in
-// common.cuh) before its first global-memory access.  Only the GEMM launches use it.  A dependent grid that starts early
-// lands on the SMs that free up first; kernels with several CTAs per SM then pile onto those SMs and run unbalanced.  The
-// GEMM runs one CTA per SM, and what the early start hides is its prologue (barrier init, descriptor prefetch).
+// common.cuh) before its first global-memory access.  Only the GEMM launches use it, including those planned at two CTAs
+// per SM: an early-started grid lands on the SMs that free up first, which can unbalance a kernel running several CTAs per
+// SM, but on the bench step (H100 SXM, 700 W) turning PDL off for the two-CTA launches changed throughput by less than
+// the run-to-run spread of about 0.2 images/s, so every GEMM keeps it.  What the
+// early start hides is the prologue (barrier init, descriptor prefetch).
 template <typename... KArgs, typename... Args>
 static inline void launch_k_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
     cudaLaunchConfig_t cfg;

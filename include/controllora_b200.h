@@ -91,6 +91,10 @@ typedef struct {
 int cl_gemm(const cl_gemm_args* args, void* stream);
 /* Split count cl_gemm's heuristic recommends for these arguments (1 = none); size split_ws with it. */
 int cl_gemm_split_hint(const cl_gemm_args* args);
+/* The plan cl_gemm makes for these arguments, without launching: info[0] = tile width (block_n), info[1] = K splits,
+   info[2] = CTAs per SM the kernel is launched for (1 or 2, chosen from the shape), info[3] = CTAs of that kernel the
+   device keeps resident per SM at the shared-memory size of the launch (cudaOccupancyMaxActiveBlocksPerMultiprocessor). */
+int cl_gemm_plan(const cl_gemm_args* args, int32_t info[4]);
 
 /* ------------------------------------------------------------------------------------------------------------
  * K2: fused attention  O = softmax(Q K^T * scale) V  per (batch, head), probabilities never leave the SM.

@@ -196,6 +196,42 @@ def resident_short_k():
         assert e < 4e-3 and e_t < 1e-4 and lora_only < 3e-2
 
 
+@case
+def two_cta_plain():
+    """short-K shapes the planner runs two CTAs per SM (BN 128), one with an M that is not a multiple of 128"""
+    _run_plain(16384, 384, 320)
+    _run_plain(32700, 384, 320)
+
+
+@case
+def two_cta_epilogue():
+    """two CTAs per SM with bias + row bias + residual, in bf16 and fp32 output"""
+    torch = _setup()
+    from controllora_b200 import ops
+
+    M, N, K = 16384, 384, 320
+    a = torch.randn(M, K, device="cuda").to(torch.bfloat16)
+    b = (torch.randn(N, K, device="cuda") / K**0.5).to(torch.bfloat16)
+    bias = torch.randn(N, device="cuda")
+    rb = torch.randn(8, N, device="cuda")
+    res = torch.randn(M, N, device="cuda").to(torch.bfloat16)
+    ref = _gemm_ref(a, b) + bias + rb.repeat_interleave(M // 8, 0) + res.float()
+    out = ops.gemm(a, b, bias=bias, row_bias=rb, rows_per_group=M // 8, residual=res)
+    out32 = ops.gemm(a, b, bias=bias, row_bias=rb, rows_per_group=M // 8, residual=res, out_fp32=True)
+    torch.cuda.synchronize()
+    print(f"two-CTA epilogue bf16 rel={_rel(out, ref):.3e}  fp32 rel={_rel(out32, ref):.3e}")
+    assert _rel(out, ref) < 4e-3 and _rel(out32, ref) < 1e-5
+
+
+@case
+def two_cta_conv():
+    """hint-encoder 3x3 convs at two CTAs per SM: 32 channels (BK 32) at BN 32 and 64, 64 channels at BN 128, stride 2"""
+    _conv_case(2, 256, 256, 32, 32, 1, 1, True)
+    _conv_case(2, 256, 256, 32, 64, 1, 1, False)
+    _conv_case(8, 128, 128, 64, 128, 1, 1, True)
+    _conv_case(2, 512, 512, 32, 32, 2, 0, False)
+
+
 def _conv_case(n, H, W, Cc, N, stride, pad_lo, with_epi):
     torch = _setup()
     import torch.nn.functional as F
