@@ -1,7 +1,8 @@
 // K2 (backward) — flash-attention backward for sm_90a on wgmma, what torch autograd derives for the reference's baddbmm /
 // softmax / bmm (models.py:140-141, 270-271, 407-408).  P is recomputed from Q, K and the forward's log2-domain LSE;
 // delta = rowsum(dO * O) comes from a small kernel first.  Both kernels use three warpgroups: a TMA producer (one elected
-// thread: the CTA's own tiles once, then a three-stage mbarrier ring of the streamed tiles) and two consumer warpgroups of
+// thread: the CTA's own tiles once, then a three-stage mbarrier ring of the streamed tiles; in the dKV kernel a second
+// warp stages each streamed query tile's lse and delta into the same ring) and two consumer warpgroups of
 // 64 rows each, whose products run on wgmma with the accumulators in registers and P / dS fed back as register A operands.
 //
 //   dKV kernel: one CTA = 128 keys of one (batch, head); it streams Q / dO tiles of 64 queries (32 for heads wider than 64):
@@ -45,10 +46,12 @@ struct BwdCfg {
     static constexpr int IN_BYTES = DCH * BI * 128;        // one streamed tile
     static constexpr int STAGE_BYTES = 2 * IN_BYTES;
     static constexpr int STAGES = 3;                       // a stage stays busy until the next tile's S has retired
-    static constexpr int SMEM_BYTES = 1024 + 2 * FIX_BYTES + STAGES * STAGE_BYTES + 256;
+    static constexpr int STAT_BYTES = 2 * BI * 4;          // dKV: lse and delta of a streamed tile's queries, per stage
+    static constexpr int SMEM_BYTES = 1024 + 2 * FIX_BYTES + STAGES * (STAGE_BYTES + STAT_BYTES) + 256;
 };
 
 // the shared producer: fixed tiles f0 / f1 (128 rows from frow0) once, then n tiles of BI rows of s0 / s1 through the ring
+// (one elected thread of warp 0)
 template <int D16>
 __device__ __forceinline__ void bwd_produce(const CUtensorMap* f0, const CUtensorMap* f1, int frow0, const CUtensorMap* s0,
                                             const CUtensorMap* s1, int n, uint8_t* sfix, uint8_t* sin, uint64_t* fix_bar,
@@ -69,19 +72,46 @@ __device__ __forceinline__ void bwd_produce(const CUtensorMap* f0, const CUtenso
     }
 }
 
-#define BWD_PROLOGUE                                                                                                     \
+// dKV: warp 1 of the producer warpgroup stages lse and delta of every streamed query tile into the ring (sstat, BI of
+// each per stage), with padding queries (>= Nq) set to lse = +inf (so P = 0) and delta = 0.  Each lane arrives on full_bar
+// after its stores.
+template <int D16>
+__device__ __forceinline__ void bwd_produce_stats(const AttnBwdParams& p, int n, float* sstat, uint64_t* full_bar,
+                                                  uint64_t* empty_bar, int h, int b, int lane) {
+    using Cfg = BwdCfg<D16>;
+    constexpr int BI = Cfg::BI;
+    const float* glse = p.lse + ((long long)b * p.H + h) * p.Nq;
+    const float* gdelta = p.delta + ((long long)b * p.H + h) * p.Nq;
+    int stage = 0; uint32_t phase = 0;
+    for (int j = 0; j < n; ++j) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        float* st = sstat + stage * (2 * BI);
+#pragma unroll 1
+        for (int i = lane; i < BI; i += 32) {
+            const int qq = j * BI + i;
+            st[i] = (qq < p.Nq) ? __ldg(glse + qq) : INFINITY;
+            st[BI + i] = (qq < p.Nq) ? __ldg(gdelta + qq) : 0.f;
+        }
+        mbar_arrive(&full_bar[stage]);
+        if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+    }
+}
+
+// FULL_COUNT: arrivals that complete a ring stage besides the TMA bytes (the TMA thread, plus 32 lanes staging lse / delta)
+#define BWD_PROLOGUE(FULL_COUNT)                                                                                         \
     extern __shared__ __align__(1024) uint8_t smem_raw[];                                                                \
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));      \
     uint8_t* sfix = smem;                                                                                                \
     uint8_t* sin = sfix + 2 * Cfg::FIX_BYTES;                                                                            \
-    uint64_t* fix_bar = reinterpret_cast<uint64_t*>(sin + Cfg::STAGES * Cfg::STAGE_BYTES);                               \
+    float* sstat = reinterpret_cast<float*>(sin + Cfg::STAGES * Cfg::STAGE_BYTES);                                       \
+    uint64_t* fix_bar = reinterpret_cast<uint64_t*>(sstat + Cfg::STAGES * 2 * Cfg::BI);                                  \
     uint64_t* full_bar = fix_bar + 1;                                                                                    \
     uint64_t* empty_bar = full_bar + Cfg::STAGES;                                                                        \
     const int warp_idx = uniform_warp_idx(), lane = threadIdx.x & 31;                                                    \
     const int wg = warp_idx >> 2;                                                                                        \
     if (threadIdx.x == 0) {                                                                                              \
         mbar_init(fix_bar, 1);                                                                                           \
-        for (int i = 0; i < Cfg::STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 2); }              \
+        for (int i = 0; i < Cfg::STAGES; ++i) { mbar_init(&full_bar[i], FULL_COUNT); mbar_init(&empty_bar[i], 2); }     \
         fence_barrier_init();                                                                                            \
     }                                                                                                                    \
     __syncthreads();                                                                                                     \
@@ -89,13 +119,11 @@ __device__ __forceinline__ void bwd_produce(const CUtensorMap* f0, const CUtenso
 
 // one dKV consumer warpgroup (keys row0 .. row0 + 63 of the CTA's 128) for output chunks [C0, C0 + NC), the last NL wide
 template <int D16, int C0, int NC, int NL>
-__device__ __forceinline__ void dkv_consume(const AttnBwdParams& p, uint8_t* sfix, uint8_t* sin, uint64_t* fix_bar,
-                                            uint64_t* full_bar, uint64_t* empty_bar, int h, int b, int k0, int nqb, int row0,
-                                            int lane, int w4) {
+__device__ __forceinline__ void dkv_consume(const AttnBwdParams& p, uint8_t* sfix, uint8_t* sin, const float* sstat,
+                                            uint64_t* fix_bar, uint64_t* full_bar, uint64_t* empty_bar, int h, int b, int k0,
+                                            int nqb, int row0, int lane, int w4) {
     using Cfg = BwdCfg<D16>;
     constexpr int BI = Cfg::BI, ACC = 32 * (NC - 1) + NL / 2;   // accumulator registers per thread of dK (and of dV)
-    const float* glse = p.lse + ((long long)b * p.H + h) * p.Nq;
-    const float* gdelta = p.delta + ((long long)b * p.H + h) * p.Nq;
     float dk[NC][32], dv[NC][32];
 #pragma unroll
     for (int c = 0; c < NC; ++c)
@@ -113,30 +141,27 @@ __device__ __forceinline__ void dkv_consume(const AttnBwdParams& p, uint8_t* sfi
         wgmma_fence();
         att_abt_issue<D16, 128, BI>(s, k_addr, row0, q_addr);     // S^T[64 keys][BI queries]
         att_abt_issue<D16, 128, BI>(dp, v_addr, row0, do_addr);   // dP^T = V dO^T
-        float lse_c[BI / 4], dl_c[BI / 4];                      // this lane's query columns 8nt + 2(lane%4) + {0,1}
-#pragma unroll
-        for (int nt = 0; nt < BI / 8; ++nt)
-#pragma unroll
-            for (int c = 0; c < 2; ++c) {
-                const int qq = j * BI + nt * 8 + 2 * (lane & 3) + c;
-                lse_c[nt * 2 + c] = (qq < p.Nq) ? __ldg(glse + qq) : INFINITY;     // P = 0 for padding queries
-                dl_c[nt * 2 + c] = (qq < p.Nq) ? __ldg(gdelta + qq) : 0.f;
-            }
+        // this lane's query columns 8nt + 2(lane%4) + {0,1} of the tile's lse and delta, as float2 pairs
+        const uint32_t stat_addr = smem_u32(sstat + stage * (2 * BI)) + 8 * (lane & 3);
         wgmma_wait<1>();                                          // S^T, and the previous tile's dK, have retired
         wgmma_fence_acc(s);
         if (j > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
 #pragma unroll
-        for (int nt = 0; nt < BI / 8; ++nt)
+        for (int nt = 0; nt < BI / 8; ++nt) {
+            const float2 l2 = ld_shared_f2(stat_addr + nt * 32);
 #pragma unroll
-            for (int c = 0; c < 4; ++c) s[nt * 4 + c] = fast_exp2(s[nt * 4 + c] * p.scale_log2 - lse_c[nt * 2 + (c & 1)]);
+            for (int c = 0; c < 4; ++c) s[nt * 4 + c] = fast_exp2(s[nt * 4 + c] * p.scale_log2 - ((c & 1) ? l2.y : l2.x));
+        }
         acc_to_a<BI / 8>(s, pa);
         att_pv_issue<NC, NL, BI, BI / 16>(dv, pa, do_addr, C0);  // dV += P^T dO
         wgmma_wait<1>();                                          // dP^T has retired
         wgmma_fence_acc(dp);
 #pragma unroll
-        for (int nt = 0; nt < BI / 8; ++nt)
+        for (int nt = 0; nt < BI / 8; ++nt) {
+            const float2 d2 = ld_shared_f2(stat_addr + BI * 4 + nt * 32);
 #pragma unroll
-            for (int c = 0; c < 4; ++c) dp[nt * 4 + c] = s[nt * 4 + c] * (dp[nt * 4 + c] - dl_c[nt * 2 + (c & 1)]);
+            for (int c = 0; c < 4; ++c) dp[nt * 4 + c] = s[nt * 4 + c] * (dp[nt * 4 + c] - ((c & 1) ? d2.y : d2.x));
+        }
         acc_to_a<BI / 8>(dp, dsa);
         att_pv_issue<NC, NL, BI, BI / 16>(dk, dsa, q_addr, C0);  // dK += dS^T Q
         // dV retires.  dK stays in flight into the next tile where its accumulators are small enough (ptxas -v: with
@@ -160,7 +185,7 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     pdl_launch_dependents();
     using Cfg = BwdCfg<D16>;
     constexpr int DCH = Cfg::DCH, BI = Cfg::BI;
-    BWD_PROLOGUE
+    BWD_PROLOGUE(33)
     int bid = blockIdx.x;
     const int kb = bid % p.num_blocks; bid /= p.num_blocks;
     const int h = bid % p.H, b = bid / p.H;
@@ -170,17 +195,19 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
         setmaxnreg_dec<40>();
         if (warp_idx == 0 && elect_one_sync())
             bwd_produce<D16>(&tmK, &tmV, k0, &tmQ, &tmDO, nqb, sfix, sin, fix_bar, full_bar, empty_bar, h, b);
+        else if (warp_idx == 1)
+            bwd_produce_stats<D16>(p, nqb, sstat, full_bar, empty_bar, h, b, lane);
         return;
     }
     setmaxnreg_inc<232>();
     const int row0 = (wg - 1) * 64, w4 = warp_idx & 3;
     // the column split is per CTA and uniform, so each side is its own fully unrolled instance
     if (DCH <= 2)
-        dkv_consume<D16, 0, DCH, head_last_n<D16>()>(p, sfix, sin, fix_bar, full_bar, empty_bar, h, b, k0, nqb, row0, lane, w4);
+        dkv_consume<D16, 0, DCH, head_last_n<D16>()>(p, sfix, sin, sstat, fix_bar, full_bar, empty_bar, h, b, k0, nqb, row0, lane, w4);
     else if (blockIdx.y == 0)
-        dkv_consume<D16, 0, 2, 64>(p, sfix, sin, fix_bar, full_bar, empty_bar, h, b, k0, nqb, row0, lane, w4);
+        dkv_consume<D16, 0, 2, 64>(p, sfix, sin, sstat, fix_bar, full_bar, empty_bar, h, b, k0, nqb, row0, lane, w4);
     else
-        dkv_consume<D16, 2, 1, head_last_n<D16>()>(p, sfix, sin, fix_bar, full_bar, empty_bar, h, b, k0, nqb, row0, lane, w4);
+        dkv_consume<D16, 2, 1, head_last_n<D16>()>(p, sfix, sin, sstat, fix_bar, full_bar, empty_bar, h, b, k0, nqb, row0, lane, w4);
 }
 
 template <int D16>
@@ -190,7 +217,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     pdl_launch_dependents();
     using Cfg = BwdCfg<D16>;
     constexpr int BI = Cfg::BI, DCH = Cfg::DCH;
-    BWD_PROLOGUE
+    BWD_PROLOGUE(1)
     int bid = blockIdx.x;
     const int qb = bid % p.num_blocks; bid /= p.num_blocks;
     const int h = bid % p.H, b = bid / p.H;
@@ -218,6 +245,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 #pragma unroll
         for (int i = 0; i < 32; ++i) dq[c][i] = 0.f;
     uint32_t dsa[BI / 16][4];                                     // dS operand of the dQ product in flight
+    const bool ragged = (p.Nk % BI) != 0;
     mbar_wait(fix_bar, 0);
     const uint32_t q_addr = smem_u32(sfix), do_addr = q_addr + Cfg::FIX_BYTES;
     int stage = 0, prev = 0; uint32_t phase = 0;
@@ -233,12 +261,14 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         wgmma_fence_acc(s);
         if (j > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
 #pragma unroll
-        for (int nt = 0; nt < BI / 8; ++nt)
+        for (int i = 0; i < BI / 2; ++i) s[i] = fast_exp2(s[i] * p.scale_log2 - lse[(i >> 1) & 1]);
+        if (ragged && j == nkb - 1) {                             // keys beyond Nk occur in the last tile only
 #pragma unroll
-            for (int c = 0; c < 4; ++c) {
-                const int key = j * BI + nt * 8 + 2 * (lane & 3) + (c & 1);
-                s[nt * 4 + c] = (key < p.Nk) ? fast_exp2(s[nt * 4 + c] * p.scale_log2 - lse[c >> 1]) : 0.f;
-            }
+            for (int nt = 0; nt < BI / 8; ++nt)
+#pragma unroll
+                for (int c = 0; c < 4; ++c)
+                    if (j * BI + nt * 8 + 2 * (lane & 3) + (c & 1) >= p.Nk) s[nt * 4 + c] = 0.f;
+        }
         wgmma_wait<0>();                                          // dP has retired
         wgmma_fence_acc(dp);
 #pragma unroll

@@ -7,10 +7,11 @@
 // One CTA = one (batch, head, 128-query block), three warpgroups:
 //   warpgroup 0    TMA producer (one elected thread): Q once, then a two-stage mbarrier ring of K / V tiles of BN keys
 //                  (4-D tensor maps {d, H, N, B}; the head dim is padded to a multiple of 64 by TMA zero fill, and
-//                  S = Q K^T runs over ceil(d / 16) K16 steps only)
+//                  S = Q K^T runs over ceil(d / 16) K16 steps only, and O += P V over ceil(d / 16) * 16 columns)
 //   warpgroups 1-2 64 query rows each: S = Q K^T with wgmma from shared memory, online softmax in the exp2 domain on the
 //                  accumulator registers (one row's statistics shared by the 4 lanes of a quad), O += P V with P as the
-//                  register A operand and V read MN-major, O kept in registers.
+//                  register A operand and V read MN-major, O kept in registers.  The warpgroups take turns (named
+//                  barriers 1 and 2) to issue S, so one warpgroup's softmax runs while the other's MMAs do.
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -92,30 +93,46 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
 
     setmaxnreg_inc<232>();
     const int row0 = (wg - 1) * 64, w4 = warp_idx & 3;
+    // Ping-pong: the two warpgroups take turns to issue S = Q K^T, so that one warpgroup's softmax runs while the other's
+    // MMAs do.  Named barrier wg (1 or 2) opens this warpgroup's turn: it completes with this warpgroup's sync and the other
+    // warpgroup's arrive at the end of its own turn.
+    const int bar_me = wg, bar_other = 3 - wg;
     float o[DCH][32];
 #pragma unroll
     for (int c = 0; c < DCH; ++c)
 #pragma unroll
         for (int i = 0; i < 32; ++i) o[c][i] = 0.f;
     float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+    if (wg == 2) named_bar_arrive(1, 256);                   // warpgroup 1 takes the first turn
     mbar_wait(q_bar, 0);
     const uint32_t q_addr = smem_u32(sq);
+    const bool ragged = (p.Nk % BN) != 0;
     int stage = 0; uint32_t phase = 0;
     for (int j = 0; j < nkb; ++j) {
         mbar_wait(&full_bar[stage], phase);
         const uint32_t k_addr = smem_u32(skv + stage * Cfg::STAGE_BYTES), v_addr = k_addr + Cfg::KV_BYTES;
         float s[BN / 2];
-        att_abt<D16, 128, BN>(s, q_addr, row0, k_addr);
-        // scaled scores in the log2 domain, keys beyond Nk masked; s[nt*4 + c]: row lane/4 + 8(c/2), key 8nt + 2(lane%4) + c%2
+        // this warpgroup's turn to issue S (see above)
+        named_bar_sync(bar_me, 256);
+        wgmma_fence();
+        att_abt_issue<D16, 128, BN>(s, q_addr, row0, k_addr);
+        named_bar_arrive(bar_other, 256);
+        wgmma_wait<0>();
+        wgmma_fence_acc(s);
+        // scaled scores in the log2 domain; s[nt*4 + c]: row lane/4 + 8(c/2), key 8nt + 2(lane%4) + c%2.  Keys beyond Nk
+        // occur in the last tile only and are masked there.
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) s[i] *= p.scale_log2;
+        if (ragged && j == nkb - 1) {
+#pragma unroll
+            for (int nt = 0; nt < BN / 8; ++nt)
+#pragma unroll
+                for (int c = 0; c < 4; ++c)
+                    if (j * BN + nt * 8 + 2 * (lane & 3) + (c & 1) >= p.Nk) s[nt * 4 + c] = -INFINITY;
+        }
         float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-        for (int nt = 0; nt < BN / 8; ++nt)
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-                const int key = j * BN + nt * 8 + 2 * (lane & 3) + (c & 1);
-                s[nt * 4 + c] = (key < p.Nk) ? s[nt * 4 + c] * p.scale_log2 : -INFINITY;
-                mx[c >> 1] = fmaxf(mx[c >> 1], s[nt * 4 + c]);
-            }
+        for (int i = 0; i < BN / 2; ++i) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s[i]);
         float corr[2], m_use[2];
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
@@ -143,10 +160,11 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
                 o[c][jj * 4] *= corr[0]; o[c][jj * 4 + 1] *= corr[0];
                 o[c][jj * 4 + 2] *= corr[1]; o[c][jj * 4 + 3] *= corr[1];
             }
-        att_pv<DCH, 64, BN, BN / 16>(o, pa, v_addr, 0);
+        att_pv<DCH, head_last_n<D16>(), BN, BN / 16>(o, pa, v_addr, 0);
         if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[stage]);
         if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
     }
+    if (wg == 1) named_bar_sync(1, 256);                     // the sync that matches warpgroup 2's last arrive
     // epilogue: O / l, bf16 store, log2-domain LSE
     float inv[2];
 #pragma unroll

@@ -76,14 +76,6 @@ __device__ __forceinline__ void att_abt_issue(float (&s)[N / 2], uint32_t a_base
     wgmma_commit();
 }
 
-template <int D16, int AR, int N>
-__device__ __forceinline__ void att_abt(float (&s)[N / 2], uint32_t a_base, int a_row0, uint32_t b_base) {
-    wgmma_fence();
-    att_abt_issue<D16, AR, N>(s, a_base, a_row0, b_base);
-    wgmma_wait<0>();
-    wgmma_fence_acc(s);
-}
-
 // issue (fence, one commit group, no wait) o[oc] += P V[:, chunk c0 + oc] for NC output chunks, the last one NL columns
 // wide: P = KC*16 columns of bf16 A fragments in registers (k = rows of the VR-row tile v), v read MN-major.  pa and o
 // must not be touched until the group has retired.
@@ -108,6 +100,12 @@ __device__ __forceinline__ void att_pv(float (&o)[NC][32], const uint32_t (&pa)[
     wgmma_wait<0>();
 #pragma unroll
     for (int oc = 0; oc < NC; ++oc) wgmma_fence_acc(o[oc]);
+}
+
+__device__ __forceinline__ float2 ld_shared_f2(uint32_t addr) {
+    float2 v;
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
+    return v;
 }
 
 // bf16 A fragments (K16 chunks) of a 64 x (NT*8) accumulator block: accumulator column block nt holds k = 8nt .. 8nt + 7
