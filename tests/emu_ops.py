@@ -532,7 +532,13 @@ def sumsq(x, out):
     out += (x.double() ** 2).sum().float()
 
 
+def _f32(x) -> float:
+    return float(torch.tensor(float(x), dtype=torch.float32))
+
+
 def _adamw(p, g, m, v, lr, beta1, beta2, eps, wd, step, gnorm_sq, max_norm, grad_scale, zero_grad):
+    # the kernels take the hyper-parameters as C floats: 1 - 0.999f is 1.3e-5 (relative) away from 1e-3
+    lr, beta1, beta2, eps, wd, max_norm, grad_scale = map(_f32, (lr, beta1, beta2, eps, wd, max_norm, grad_scale))
     coef = float(grad_scale)
     if gnorm_sq is not None and max_norm > 0:
         total = math.sqrt(float(gnorm_sq)) * grad_scale
