@@ -10,9 +10,11 @@ from .vae import AutoencoderKL
 from .clip import CLIPTextModel
 from .annotator import CannyDetector, canny_batch
 from .transforms import HWC3, reference_crops, resize_image, train_transform
+from .pose import draw_bodypose, pose_batch, pose_control
 
 __all__ = [
     "ControlLoRA", "ControlLoRAOutput", "ControlLoRACrossAttnProcessor", "ControlLoRACrossAttnProcessorV2",
     "LoRACrossAttnProcessor", "LoRALinearLayer", "UNet2DConditionModel", "AutoencoderKL", "CLIPTextModel",
     "CannyDetector", "canny_batch", "HWC3", "reference_crops", "resize_image", "train_transform",
+    "draw_bodypose", "pose_batch", "pose_control",
 ]

@@ -41,6 +41,10 @@ def lib() -> C.CDLL:
         _lib.cl_resample.restype = C.c_int
         _lib.cl_resample.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
                                      C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        _lib.cl_pose_render.restype = C.c_int
+        _lib.cl_pose_render.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                        C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int,
+                                        C.c_void_p, C.c_void_p, C.c_void_p]
     return _lib
 
 
@@ -150,6 +154,35 @@ class ResampleDesc(C.Structure):
         ("tab1", C.c_int32), ("k1", C.c_int32), ("tab2", C.c_int32), ("k2", C.c_int32),
         ("op", C.c_int32),
         ("scale", C.c_float),
+        ("pad_", C.c_int32),
+    ]
+
+
+class PoseImage(C.Structure):
+    """cl_pose_image"""
+    _fields_ = [
+        ("bg_off", C.c_int64),
+        ("Hc", C.c_int32), ("Wc", C.c_int32),
+        ("y0", C.c_int32), ("x0", C.c_int32), ("h", C.c_int32), ("w", C.c_int32),
+        ("circle0", C.c_int32), ("n_circles", C.c_int32),
+        ("limb0", C.c_int32), ("n_limbs", C.c_int32),
+    ]
+
+
+class PoseCircle(C.Structure):
+    """cl_pose_circle"""
+    _fields_ = [("x", C.c_int32), ("y", C.c_int32), ("color", C.c_int32), ("pad_", C.c_int32)]
+
+
+class PoseLimb(C.Structure):
+    """cl_pose_limb"""
+    _fields_ = [
+        ("mask_off", C.c_int64),
+        ("image", C.c_int32),
+        ("cx", C.c_int32), ("cy", C.c_int32),
+        ("half_len", C.c_int32), ("angle", C.c_int32),
+        ("color", C.c_int32),
+        ("bx0", C.c_int32), ("by0", C.c_int32), ("bw", C.c_int32), ("bh", C.c_int32),
         ("pad_", C.c_int32),
     ]
 

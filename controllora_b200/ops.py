@@ -820,3 +820,36 @@ def resample(filter_id: int, desc, packed: torch.Tensor, src: torch.Tensor, tmp:
                                  tables.numel(), _ptr(tmp), tmp.numel(), out_h, out_w, _ptr(out_nchw), _ptr(out_nhwc),
                                  _stream()), "cl_resample")
     return out_nchw, out_nhwc
+
+
+def pose_render(img, circles, limbs, packed: torch.Tensor, mask: torch.Tensor, out_h: int, out_w: int, *, flip: bool = True,
+                bg=None, out_canvas=None, out_guide=None):
+    """cl_pose_render: `img`, `circles`, `limbs` are ctypes arrays of _lib.PoseImage / PoseCircle / PoseLimb (host copies,
+    validated by the launcher); `packed` the uint8 device buffer holding the same bytes back to back (one upload);
+    `mask` int32 scratch for the limbs' coverage bitmasks; `bg` the uint8 background canvases back to back.  Fills
+    out_canvas uint8 [B, out_h, out_w, 3] and / or out_guide fp32 [B, 3, out_h, out_w]."""
+    _req(packed, torch.uint8, "packed")
+    _req(mask, torch.int32, "mask")
+    B, nc, nl = len(img), len(circles), len(limbs)
+    sizes = [C.sizeof(_lib.PoseImage) * B, C.sizeof(_lib.PoseCircle) * nc, C.sizeof(_lib.PoseLimb) * nl]
+    if packed.numel() < sum(sizes):
+        raise _lib.CLError(f"packed: {packed.numel()} bytes cannot hold the {sum(sizes)}-byte descriptors")
+    for name, t, dtype, shape in (("out_canvas", out_canvas, torch.uint8, (B, out_h, out_w, 3)),
+                                  ("out_guide", out_guide, torch.float32, (B, 3, out_h, out_w))):
+        if t is None:
+            continue
+        _req(t, dtype, name)
+        if tuple(t.shape) != shape or not t.is_contiguous():
+            raise _lib.CLError(f"{name}: expected a contiguous {shape} tensor, got shape {tuple(t.shape)}")
+    if bg is not None:
+        _req(bg, torch.uint8, "bg")
+    for name, t in (("mask", mask), ("bg", bg), ("out_canvas", out_canvas), ("out_guide", out_guide)):
+        if t is not None and (t.device != packed.device or not t.is_contiguous()):
+            raise _lib.CLError(f"{name}: must be contiguous and on {packed.device}")
+    base = packed.data_ptr()
+    dev = [C.c_void_p(base), C.c_void_p(base + sizes[0]), C.c_void_p(base + sizes[0] + sizes[1])]
+    check(_lib.lib().cl_pose_render(C.cast(img, C.c_void_p), dev[0], B, C.cast(circles, C.c_void_p), dev[1], nc,
+                                    C.cast(limbs, C.c_void_p), dev[2], nl, _ptr(bg), 0 if bg is None else bg.numel(),
+                                    _ptr(mask), mask.numel(), out_h, out_w, int(flip), _ptr(out_canvas), _ptr(out_guide),
+                                    _stream()), "cl_pose_render")
+    return out_canvas, out_guide

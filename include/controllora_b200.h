@@ -376,6 +376,54 @@ int cl_resample(int filter, const cl_resample_desc* desc, const cl_resample_desc
                 int64_t src_bytes, const int32_t* tables, int64_t table_len, int32_t* tmp, int64_t tmp_len, int out_h,
                 int out_w, float* out_nchw, uint8_t* out_nhwc, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * K11: OpenPose body-skeleton renderer for a ragged batch, bit for bit with the reference's draw_bodypose
+ * (annotator/openpose/util.py:37-70) and the guide arithmetic around it: annotator/openpose/__init__.py:27-33
+ * (OpenposeDetector: zero canvas), apps/gradio_pose2image.py:70-78 (INTER_NEAREST resize, channel flip, / 127.5 - 1),
+ * process/mpii_pose.py:29-44 (crop of the drawn guide, / 127.5 - 1).
+ * Per image: a canvas Hc x Wc (zeros, or a caller's uint8 [Hc, Wc, 3] background), its circles and limbs in draw order,
+ * and an output window: crop (y0, x0, h, w) of the canvas, resized with cv2 INTER_NEAREST to out_h x out_w.
+ *   circles: cv2.circle(canvas, (x, y), 4, colour, -1), written over the canvas.
+ *   limbs:   cv2.fillConvexPoly(cur, cv2.ellipse2Poly((cx, cy), (half_len, 4), angle, 0, 360, 1), colour) blended with
+ *            cv2.addWeighted(canvas, 0.4, cur, 0.6, 0).  The host computes the integer ellipse parameters (Python
+ *            floats, the reference's operations) and a conservative box; the polygon, its edge lines and its scanline
+ *            fill are built on the device into a coverage bitmask per limb (mask, bh rows of (bw + 31) / 32 words).
+ *   img / circles / limbs: on the host (validated) and the same bytes on the device (_dev).  A limb slot with
+ *            image = -1 is unused, so a fixed-capacity buffer can be refilled and a captured graph replayed.
+ *   outputs (at least one, NULL = skip): out_canvas uint8 [B, out_h, out_w, 3], channels in drawing order (OpenCV's
+ *            BGR); out_guide fp32 [B, 3, out_h, out_w] = x / 127.5 - 1 with each operation rounded to fp32, channels
+ *            reversed when flip = 1 (the app's detected_map[..., ::-1]).
+ * Two launches whatever the data, no host synchronisation.
+ * ---------------------------------------------------------------------------------------------------------- */
+typedef struct {
+    int64_t bg_off;               /* byte offset of the background [Hc, Wc, 3] in bg; -1: a zero canvas */
+    int32_t Hc, Wc;               /* canvas size */
+    int32_t y0, x0, h, w;         /* crop window of the canvas, resized to the output size */
+    int32_t circle0, n_circles;   /* its circles: circles[circle0 .. circle0 + n_circles), in draw order */
+    int32_t limb0, n_limbs;       /* its limbs, likewise */
+} cl_pose_image;
+
+typedef struct {
+    int32_t x, y;                 /* centre (int(x), int(y)) */
+    int32_t color;                /* c0 | c1 << 8 | c2 << 16, channels in drawing order */
+    int32_t pad_;
+} cl_pose_circle;
+
+typedef struct {
+    int64_t mask_off;             /* word offset of its coverage bitmask in mask */
+    int32_t image;                /* its image, -1: unused slot */
+    int32_t cx, cy;               /* ellipse centre (int(mY), int(mX)) of util.py:65 */
+    int32_t half_len, angle;      /* int(length / 2), int(angle) */
+    int32_t color;                /* as cl_pose_circle.color */
+    int32_t bx0, by0, bw, bh;     /* coverage box in canvas pixels, inside the canvas; bw = bh = 0: off the canvas */
+    int32_t pad_;
+} cl_pose_limb;
+
+int cl_pose_render(const cl_pose_image* img, const cl_pose_image* img_dev, int B, const cl_pose_circle* circles,
+                   const cl_pose_circle* circles_dev, int n_circles, const cl_pose_limb* limbs, const cl_pose_limb* limbs_dev,
+                   int n_limbs, const uint8_t* bg, int64_t bg_bytes, uint32_t* mask, int64_t mask_words, int out_h, int out_w,
+                   int flip, uint8_t* out_canvas, float* out_guide, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
