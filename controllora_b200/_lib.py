@@ -45,6 +45,9 @@ def lib() -> C.CDLL:
         _lib.cl_pose_render.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
                                         C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int,
                                         C.c_void_p, C.c_void_p, C.c_void_p]
+        _lib.cl_cfg_plms_step_dev.restype = C.c_int
+        _lib.cl_cfg_plms_step_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                              C.c_float, C.c_void_p]
     return _lib
 
 

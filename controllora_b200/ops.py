@@ -729,6 +729,19 @@ def cfg_solver_step_dev(eps2, latents, x0_prev, coef, step_ctr, guidance: float,
           C.c_float(guidance), int(kind))
 
 
+def cfg_plms_step_dev(eps2, latents, ring, saved, rows, step_ctr, guidance: float):
+    """CFG + PNDM (PLMS) update with the step's row read from rows[*step_ctr] (sampler.pndm_rows); updates the eps ring
+    [3, *latents.shape], the saved sample and the latents in place and advances the device step counter, in one launch.
+    eps2 [2B, ...] fp32 = [uncond | cond]."""
+    for t, name in ((eps2, "eps2"), (latents, "latents"), (ring, "ring"), (saved, "saved"), (rows, "rows")):
+        _req(t, torch.float32, name)
+        assert t.is_contiguous(), name
+    n = latents.numel()
+    assert eps2.numel() == 2 * n and ring.numel() == 3 * n and saved.numel() == n
+    assert rows.dim() == 2 and rows.shape[1] == 8 and step_ctr.dtype == torch.int64 and step_ctr.numel() == 1
+    _call("cl_cfg_plms_step_dev", _p(eps2), _p(latents), _p(ring), _p(saved), _p(rows), _p(step_ctr), n, float(guidance))
+
+
 class SkinnyQueue:
     """Collects the rank-r gradient reductions (dA / dB of every LoRA adapter) and issues them CL_SKINNY_MAX at a time
     through cl_skinny_atb_batch.  The queue keeps the operand tensors alive until the launch is enqueued."""

@@ -39,19 +39,41 @@ def ddim_coeffs(t: int, num_inference_steps: int, ac: List[float], num_train_tim
     return ac[t], (ac[prev] if prev >= 0 else ac[0])
 
 
-@torch.no_grad()
-def ddim_sample(unet, control_lora, guide: torch.Tensor, cond: torch.Tensor, uncond: torch.Tensor, num_inference_steps: int = 50,
-                guidance_scale: float = 7.5, latents: Optional[torch.Tensor] = None, seed: int = 0) -> torch.Tensor:
-    """guide [B,3,H,W] in [-1,1]; cond / uncond text states [B,77,D] bf16.  Returns the final latents [B,4,H/8,W/8] fp32."""
-    B = guide.shape[0]
-    dev = guide.device
-    h, w = guide.shape[2] // 8, guide.shape[3] // 8
+def _check_control(control_lora, guide) -> None:
+    if (control_lora is None) != (guide is None):
+        raise ValueError("pass control_lora and guide together, or neither of them (sampling without a ControlLoRA)")
+
+
+def _begin_loop(control_lora, guide, cond, uncond, latents, seed, height, width):
+    """Start of every eager loop: initial latents (seeded CPU draw unless given), `control_lora(guide)` tiled to the CFG batch
+    when there is a ControlLoRA, and the [uncond | cond] text states.  Without a ControlLoRA (control_lora = guide = None) the
+    UNet runs with whatever attention processors are installed, and the latent size comes from `latents` or height / width."""
+    _check_control(control_lora, guide)
+    ref = cond if guide is None else guide
+    B, dev = ref.shape[0], ref.device
+    if guide is not None:
+        h, w = guide.shape[2] // 8, guide.shape[3] // 8
+    elif latents is not None:
+        h, w = latents.shape[2], latents.shape[3]
+    else:
+        h, w = height // 8, width // 8
     if latents is None:
         g = torch.Generator(device="cpu").manual_seed(seed)
         latents = torch.randn(B, 4, h, w, generator=g).to(dev)
     latents = latents.float().contiguous().clone()
-    control_lora(torch.cat([guide, guide], 0))                     # inject once, for [uncond | cond]
+    if control_lora is not None:
+        control_lora(torch.cat([guide, guide], 0))                 # inject once, for [uncond | cond]
     ehs = torch.cat([uncond, cond], 0).to(torch.bfloat16).contiguous()
+    return B, dev, latents, ehs
+
+
+@torch.no_grad()
+def ddim_sample(unet, control_lora, guide: Optional[torch.Tensor], cond: torch.Tensor, uncond: torch.Tensor, num_inference_steps: int = 50,
+                guidance_scale: float = 7.5, latents: Optional[torch.Tensor] = None, seed: int = 0, height: int = 512,
+                width: int = 512) -> torch.Tensor:
+    """guide [B,3,H,W] in [-1,1]; cond / uncond text states [B,77,D] bf16.  Returns the final latents [B,4,H/8,W/8] fp32.
+    control_lora = guide = None samples without a ControlLoRA (height / width then give the image size unless latents do)."""
+    B, dev, latents, ehs = _begin_loop(control_lora, guide, cond, uncond, latents, seed, height, width)
     ac = sd15_alphas_cumprod()
     for t in ddim_timesteps(num_inference_steps):
         x2 = torch.cat([latents, latents], 0)
@@ -98,19 +120,12 @@ def dpmpp_2m_coeffs(i: int, timesteps: List[int], ac: List[float], lower_order_f
 
 
 @torch.no_grad()
-def dpmpp_sample(unet, control_lora, guide: torch.Tensor, cond: torch.Tensor, uncond: torch.Tensor, num_inference_steps: int = 30,
-                 guidance_scale: float = 7.5, latents: Optional[torch.Tensor] = None, seed: int = 0) -> torch.Tensor:
+def dpmpp_sample(unet, control_lora, guide: Optional[torch.Tensor], cond: torch.Tensor, uncond: torch.Tensor, num_inference_steps: int = 30,
+                 guidance_scale: float = 7.5, latents: Optional[torch.Tensor] = None, seed: int = 0, height: int = 512,
+                 width: int = 512) -> torch.Tensor:
     """Same contract as ddim_sample with the DPM-Solver++(2M) update; one fused CFG + solver kernel per step."""
-    B = guide.shape[0]
-    dev = guide.device
-    h, w = guide.shape[2] // 8, guide.shape[3] // 8
-    if latents is None:
-        g = torch.Generator(device="cpu").manual_seed(seed)
-        latents = torch.randn(B, 4, h, w, generator=g).to(dev)
-    latents = latents.float().contiguous().clone()
+    B, dev, latents, ehs = _begin_loop(control_lora, guide, cond, uncond, latents, seed, height, width)
     x0_prev = torch.zeros_like(latents)
-    control_lora(torch.cat([guide, guide], 0))                     # inject once, for [uncond | cond]
-    ehs = torch.cat([uncond, cond], 0).to(torch.bfloat16).contiguous()
     ac = sd15_alphas_cumprod()
     ts = dpm_timesteps(num_inference_steps)
     for i, t in enumerate(ts):
@@ -119,6 +134,71 @@ def dpmpp_sample(unet, control_lora, guide: torch.Tensor, cond: torch.Tensor, un
         eps2 = unet(x2, tt, ehs).sample
         a_s, sg_s, c_x, c_m0, c_m1 = dpmpp_2m_coeffs(i, ts, ac)
         ops.cfg_dpmpp_step(eps2, latents, x0_prev, guidance_scale, a_s, sg_s, c_x, c_m0, c_m1)
+    return latents
+
+
+# ---------------------------------------------------------------------------------------------- PNDM (PLMS)
+PLMS_PUSH, PLMS_SAVE, PLMS_RESTART = 1, 2, 4          # flag bits of a pndm_rows row (column 7)
+_PLMS_WEIGHTS = {1: (1.0,), 2: (3 / 2, -1 / 2), 3: (23 / 12, -16 / 12, 5 / 12), 4: (55 / 24, -59 / 24, 37 / 24, -9 / 24)}
+
+
+def pndm_timesteps(num_inference_steps: int, num_train_timesteps: int = 1000, steps_offset: int = 1) -> List[int]:
+    """UNet timesteps of diffusers' PNDMScheduler with skip_prk_steps (the SD-1.5 scheduler config): the DDIM grid with its
+    second timestep repeated, concat(t[:-1], t[-2:-1], t[-1:])[::-1] - N + 1 model calls (981, 961, 961, 941, ..., 1 at
+    N = 50), a single call at N = 1."""
+    ratio = num_train_timesteps // num_inference_steps
+    t = [i * ratio + steps_offset for i in range(num_inference_steps)]
+    return (t[:-1] + t[-2:-1] + t[-1:])[::-1]
+
+
+def pndm_rows(num_inference_steps: int, ac: List[float], num_train_timesteps: int = 1000) -> List[List[float]]:
+    """One row per model call of PNDMScheduler.step_plms, the program of cl_cfg_plms_step_dev:
+    [UNet timestep, sample_coeff, eps_coeff, w_new, w_1, w_2, w_3, flags].  The update is
+    x <- sample_coeff * s + eps_coeff * (w_new eps + w_1 r1 + w_2 r2 + w_3 r3), with r1..r3 the most recent pushed eps and s the
+    current sample (or the sample saved at call 0, on the restart at call 1).  Call 1 re-runs the transfer of call 0
+    (t + ratio -> t) from the saved sample with the mean of the two eps and does not push; every other call pushes its eps
+    and uses the Adams-Bashforth weights of the history length (at most 4)."""
+    ratio = num_train_timesteps // num_inference_steps
+    rows, n_ets = [], 0
+    for c, t in enumerate(pndm_timesteps(num_inference_steps, num_train_timesteps)):
+        flags = 0
+        if c != 1:
+            n_ets = min(n_ets + 1, 4)
+            flags |= PLMS_PUSH
+            t_from, t_to = t, t - ratio
+        else:
+            t_from, t_to = t + ratio, t
+        if c == 0:
+            w, flags = (1.0,), flags | PLMS_SAVE
+        elif c == 1:
+            w, flags = (0.5, 0.5), flags | PLMS_RESTART
+        else:
+            w = _PLMS_WEIGHTS[n_ets]
+        if t_from >= len(ac):          # N = 1000: the grid 1 .. 1000 leaves the table (diffusers' own index fails there too)
+            raise ValueError(f"PNDM with {num_inference_steps} steps reaches timestep {t_from}, outside the {len(ac)} training steps")
+        a_t = ac[t_from]
+        a_p = ac[t_to] if t_to >= 0 else ac[0]
+        denom = a_t * (1.0 - a_p) ** 0.5 + (a_t * (1.0 - a_t) * a_p) ** 0.5
+        rows.append([float(t), (a_p / a_t) ** 0.5, -(a_p - a_t) / denom, *(list(w) + [0.0] * (4 - len(w))), float(flags)])
+    return rows
+
+
+@torch.no_grad()
+def pndm_sample(unet, control_lora, guide: Optional[torch.Tensor], cond: torch.Tensor, uncond: torch.Tensor, num_inference_steps: int = 50,
+                guidance_scale: float = 7.5, latents: Optional[torch.Tensor] = None, seed: int = 0, height: int = 512,
+                width: int = 512) -> torch.Tensor:
+    """Same contract as ddim_sample with diffusers' PNDMScheduler (skip_prk_steps, the default scheduler of an SD-1.5
+    pipeline): N + 1 UNet calls, one fused CFG + PLMS kernel per call reading its row of `pndm_rows` through a device counter."""
+    B, dev, latents, ehs = _begin_loop(control_lora, guide, cond, uncond, latents, seed, height, width)
+    rows = torch.tensor(pndm_rows(num_inference_steps, sd15_alphas_cumprod()), dtype=torch.float32, device=dev)
+    ring = torch.zeros((3,) + tuple(latents.shape), device=dev, dtype=torch.float32)
+    saved = torch.zeros_like(latents)
+    ctr = torch.zeros(1, device=dev, dtype=torch.int64)
+    for t in pndm_timesteps(num_inference_steps):
+        x2 = torch.cat([latents, latents], 0)
+        tt = torch.full((2 * B,), float(t), device=dev)
+        eps2 = unet(x2, tt, ehs).sample
+        ops.cfg_plms_step_dev(eps2, latents, ring, saved, rows, ctr, guidance_scale)
     return latents
 
 
@@ -132,16 +212,20 @@ class GraphedSampler:
 
     Everything that does not depend on the timestep runs once per image batch, outside the graph (SURVEY f2): the hint
     encoder, LoRA operand packing, the per-level control products `u = Ac c` / v1 `t_add` tables, and the k / v projections
-    of the text states.  scheduler: "ddim" (eta = 0, config C3) or "dpmpp" (DPM-Solver++(2M), the reference's validation /
-    app scheduler, config C5)."""
+    of the text states.  scheduler: "ddim" (eta = 0, config C3), "dpmpp" (DPM-Solver++(2M), the reference's validation /
+    app scheduler, config C5) or "pndm" (PNDMScheduler with skip_prk_steps, the default scheduler of an SD-1.5 pipeline: N + 1
+    replays, with the eps history and the saved sample of its restart step in device buffers).
+
+    control_lora = None samples without a ControlLoRA: the UNet runs with whatever processors are installed (DreamBooth LoRA
+    processors, or none for the base model), there is no hint encoder and no control product, and `guide` is None."""
 
     def __init__(self, unet, control_lora, batch: int, height: int = 512, width: int = 512, scheduler: str = "ddim",
                  num_inference_steps: int = 50, guidance_scale: float = 7.5, scale: float = 1.0, text_dim: Optional[int] = None):
-        if scheduler not in ("ddim", "dpmpp"):
+        if scheduler not in ("ddim", "dpmpp", "pndm"):
             raise ValueError(f"unknown scheduler {scheduler}")
         self.unet, self.cl = unet, control_lora
         self.B, self.h, self.w = batch, height // 8, width // 8
-        self.kind = 0 if scheduler == "ddim" else 1
+        self.kind = {"ddim": 0, "dpmpp": 1, "pndm": 2}[scheduler]
         self.steps, self.guidance, self.scale = int(num_inference_steps), float(guidance_scale), float(scale)
         dev = unet.device_
         ac = sd15_alphas_cumprod()
@@ -151,20 +235,27 @@ class GraphedSampler:
             for t in ts:
                 a_t, a_p = ddim_coeffs(t, self.steps, ac)
                 rows.append([a_t ** 0.5, (1 - a_t) ** 0.5, a_p ** 0.5, (1 - a_p) ** 0.5, 0, 0, 0, 0])
-        else:
+        elif self.kind == 1:
             ts = dpm_timesteps(self.steps)
             rows = [list(dpmpp_2m_coeffs(i, ts, ac)) + [0, 0, 0] for i in range(self.steps)]
+        else:
+            ts = pndm_timesteps(self.steps)
+            rows = pndm_rows(self.steps, ac)
         self.timesteps = ts
+        self.calls = len(ts)                     # UNet calls per image batch: N, or N + 1 for PNDM
         self.ts_table = torch.tensor([float(t) for t in ts], dtype=torch.float32, device=dev)
         self.coef = torch.tensor(rows, dtype=torch.float32, device=dev).contiguous()
         B2 = 2 * batch
         td = text_dim if text_dim is not None else unet.config.cross_attention_dim
         self.latents = torch.zeros(batch, 4, self.h, self.w, device=dev, dtype=torch.float32)
         self.x0_prev = torch.zeros_like(self.latents)
+        if self.kind == 2:
+            self.ring = torch.zeros((3,) + tuple(self.latents.shape), device=dev, dtype=torch.float32)
+            self.saved = torch.zeros_like(self.latents)
         self.x2 = torch.zeros(B2, 4, self.h, self.w, device=dev, dtype=torch.float32)
         self.tt = torch.zeros(B2, device=dev, dtype=torch.float32)
         self.ehs = torch.zeros(B2, 77, td, device=dev, dtype=torch.bfloat16)
-        self.guide2 = torch.zeros(B2, 3, height, width, device=dev, dtype=torch.float32)
+        self.guide2 = None if control_lora is None else torch.zeros(B2, 3, height, width, device=dev, dtype=torch.float32)
         self.step_ctr = torch.zeros(1, device=dev, dtype=torch.int64)
         self._graph = None
         self._ctx = None
@@ -174,36 +265,44 @@ class GraphedSampler:
         ops.sampler_prep(self.latents, self.x2, self.tt, self.ts_table, self.step_ctr)
         ctx = self._ctx
         pred, _, _ = self.unet.run_engine(self.x2, self.tt, self.ehs, {}, tape=None, scale=self.scale, prepared=ctx)
-        ops.cfg_solver_step_dev(pred.data, self.latents, self.x0_prev, self.coef, self.step_ctr, self.guidance, self.kind)
+        if self.kind == 2:
+            ops.cfg_plms_step_dev(pred.data, self.latents, self.ring, self.saved, self.coef, self.step_ctr, self.guidance)
+        else:
+            ops.cfg_solver_step_dev(pred.data, self.latents, self.x0_prev, self.coef, self.step_ctr, self.guidance, self.kind)
 
     @torch.no_grad()
-    def __call__(self, guide: torch.Tensor, cond: torch.Tensor, uncond: torch.Tensor, latents: Optional[torch.Tensor] = None,
+    def __call__(self, guide: Optional[torch.Tensor], cond: torch.Tensor, uncond: torch.Tensor, latents: Optional[torch.Tensor] = None,
                  seed: int = 0, use_graph: bool = True) -> torch.Tensor:
-        """guide [B,3,H,W] in [-1,1]; cond / uncond [B,77,D].  Returns the final latents [B,4,H/8,W/8] fp32 (a view of the
-        sampler's static buffer: clone it before the next call)."""
+        """guide [B,3,H,W] in [-1,1] (None without a ControlLoRA); cond / uncond [B,77,D].  Returns the final latents
+        [B,4,H/8,W/8] fp32 (a view of the sampler's static buffer: clone it before the next call)."""
         from . import _lib
 
         B = self.B
-        assert guide.shape[0] == B
+        _check_control(self.cl, guide)
+        assert (guide if guide is not None else cond).shape[0] == B
         if latents is None:
             g = torch.Generator(device="cpu").manual_seed(seed)
             latents = torch.randn(B, 4, self.h, self.w, generator=g)
         self.latents.copy_(latents.to(self.latents.device, torch.float32))
         self.x0_prev.zero_()
+        if self.kind == 2:
+            self.ring.zero_()
+            self.saved.zero_()
         self.step_ctr.zero_()
-        self.guide2[:B].copy_(guide)
-        self.guide2[B:].copy_(guide)
         self.ehs[:B].copy_(uncond.to(torch.bfloat16))
         self.ehs[B:].copy_(cond.to(torch.bfloat16))
-        # once per image batch: hint encoder (control states into static memory), packing, u = Ac c, t_add tables
-        self.cl(self.guide2)
+        if self.cl is not None:
+            self.guide2[:B].copy_(guide)
+            self.guide2[B:].copy_(guide)
+            # once per image batch: hint encoder (control states into static memory), packing, u = Ac c, t_add tables
+            self.cl(self.guide2)
         if self._graph is None or not use_graph:
             self._ctx = self.unet.prepare_inference(self.scale)
         else:
             # the captured kernels read the addresses held by the prepared context: refresh its contents in place
             self._refresh_prepared()
         if not use_graph:
-            for _ in range(self.steps):
+            for _ in range(self.calls):
                 self._one_step()
             return self.latents
         first = 0
@@ -218,7 +317,7 @@ class GraphedSampler:
             self._graph = graph
             # the capture itself does not execute: state is after ONE eager step
             first = 1
-        for _ in range(first, self.steps):
+        for _ in range(first, self.calls):
             self._graph.replay()
         return self.latents
 
@@ -248,23 +347,72 @@ class GraphedSampler:
 
 
 @torch.no_grad()
-def generate(unet, control_lora, vae, text_encoder, guide: torch.Tensor, input_ids: torch.Tensor, uncond_input_ids: torch.Tensor,
+def generate(unet, control_lora, vae, text_encoder, guide: Optional[torch.Tensor], input_ids: torch.Tensor, uncond_input_ids: torch.Tensor,
              num_inference_steps: int = 50, guidance_scale: float = 7.5, scheduler: str = "ddim", latents: Optional[torch.Tensor] = None,
-             seed: int = 0, sampler: Optional["GraphedSampler"] = None) -> torch.Tensor:
+             seed: int = 0, sampler: Optional["GraphedSampler"] = None, height: int = 512, width: int = 512,
+             use_graph: bool = True) -> torch.Tensor:
     """What the reference's validation loop and apps ask of `StableDiffusionPipeline` after `control_lora(guide)`
     (train_text_to_image_control_lora.py:824-843, apps/gradio_*2image.py:75-89, mix_lora_and_control_lora.py:153-164), on this
     package's frozen encoders: prompt / negative-prompt token ids -> text states (`text_encoder(ids)[0]`), the CFG denoise loop
-    (`scheduler` = "ddim" or "dpmpp"; pass a `GraphedSampler` to replay the captured step instead of launching from Python), then
-    `vae.decode(latents / scaling_factor).sample` mapped from [-1, 1] to [0, 1] like the pipeline's `(image / 2 + 0.5).clamp(0, 1)`.
-    guide [B,3,H,W] in [-1,1]; ids [B,77] (tokenisation stays with the caller: the tokenizer is data-pipeline code).  Returns images
-    [B,3,H,W] fp32 in [0,1]."""
+    (`scheduler` = "ddim", "dpmpp" or "pndm"; pass a `GraphedSampler` to replay the captured step instead of launching from
+    Python), then `vae.decode(latents / scaling_factor).sample` mapped from [-1, 1] to [0, 1] like the pipeline's
+    `(image / 2 + 0.5).clamp(0, 1)`.  guide [B,3,H,W] in [-1,1]; ids [B,77] (tokenisation stays with the caller: the tokenizer is
+    data-pipeline code).  control_lora = guide = None is the pipeline without a ControlLoRA (DreamBooth validation images with
+    LoRA processors installed, train_dreambooth_lora.py:947-963; the base model's class images, :594-614); height / width then
+    give the image size unless `latents` does.  use_graph = False runs a sampler's step program without capturing it.
+    Returns images [B,3,H,W] fp32 in [0,1]."""
     cond = text_encoder(input_ids)[0]
     uncond = text_encoder(uncond_input_ids)[0]
     if sampler is not None:
-        lat = sampler(guide, cond, uncond, latents=latents, seed=seed).clone()
+        lat = sampler(guide, cond, uncond, latents=latents, seed=seed, use_graph=use_graph).clone()
     else:
-        fn = {"ddim": ddim_sample, "dpmpp": dpmpp_sample}[scheduler]
+        fn = {"ddim": ddim_sample, "dpmpp": dpmpp_sample, "pndm": pndm_sample}[scheduler]
         lat = fn(unet, control_lora, guide, cond, uncond, num_inference_steps=num_inference_steps, guidance_scale=guidance_scale,
-                 latents=latents, seed=seed)
+                 latents=latents, seed=seed, height=height, width=width)
     img = vae.decode(lat / float(vae.config.scaling_factor)).sample
     return ops.channel_affine_nchw(img.contiguous(), 0.5, torch.full((img.shape[1],), 0.5, device=img.device, dtype=torch.float32)).clamp_(0.0, 1.0)
+
+
+@torch.no_grad()
+def sample_class_images(unet, vae, text_encoder, class_ids: torch.Tensor, uncond_ids: torch.Tensor, num_images: int, out_dir,
+                        sample_batch_size: int = 4, num_inference_steps: int = 50, guidance_scale: float = 7.5, height: int = 512,
+                        width: int = 512, seed: int = 0, sampler: Optional["GraphedSampler"] = None,
+                        use_graph: bool = True) -> List[str]:
+    """The prior-preservation class images of train_dreambooth_lora.py:580-620: `out_dir` is topped up to `num_images` entries
+    (the entries already there are counted, only the missing images are generated), in batches of `sample_batch_size`, by the
+    plain SD-1.5 pipeline - no ControlLoRA, the UNet with whatever processors are installed (none, for the base model), the
+    checkpoint's own scheduler (PNDM, 50 steps, guidance 7.5) - replayed as one captured step on a GraphedSampler.  Images
+    are converted like the pipeline's numpy_to_pil, `(x * 255).round()` to uint8, and saved through Pillow as
+    `<index + existing>-<sha1 of the image bytes>.jpg`.  class_ids / uncond_ids: token ids [77] or [1, 77] of the class prompt
+    and of the empty prompt (tokenisation stays with the caller).  The latents of a batch are drawn from `seed` plus the index
+    of its first new image.  Returns the paths written."""
+    import hashlib
+    from pathlib import Path
+
+    from PIL import Image
+
+    out = Path(out_dir)
+    out.mkdir(parents=True, exist_ok=True)
+    cur = len(list(out.iterdir()))
+    todo = int(num_images) - cur
+    if todo <= 0:
+        return []
+    bs = int(sample_batch_size)
+    if sampler is None:
+        sampler = GraphedSampler(unet, None, bs, height, width, scheduler="pndm", num_inference_steps=num_inference_steps,
+                                 guidance_scale=guidance_scale)
+    elif sampler.cl is not None or sampler.B != bs:
+        raise ValueError("sample_class_images needs a GraphedSampler without a ControlLoRA, of batch sample_batch_size")
+    ids = class_ids.reshape(1, -1).expand(bs, -1).contiguous()
+    neg = uncond_ids.reshape(1, -1).expand(bs, -1).contiguous()
+    written = []
+    for start in range(0, todo, bs):
+        n = min(bs, todo - start)                  # the last batch runs full and keeps its first n images
+        img = generate(unet, None, vae, text_encoder, None, ids, neg, sampler=sampler, seed=seed + start, use_graph=use_graph)
+        arr = (img[:n].permute(0, 2, 3, 1) * 255.0).round().to(torch.uint8).cpu().numpy()
+        for i in range(n):
+            image = Image.fromarray(arr[i])
+            name = out / f"{start + i + cur}-{hashlib.sha1(image.tobytes()).hexdigest()}.jpg"
+            image.save(name)
+            written.append(str(name))
+    return written

@@ -222,6 +222,13 @@ int cl_sampler_prep(const float* latents, float* x2, float* tt, const float* ts_
                     int64_t n_half, int B2, void* stream);
 int cl_cfg_solver_step_dev(const float* eps2, float* latents, float* x0_prev, const float* coef, unsigned long long* step_ctr,
                            int64_t n_half, float guidance, int kind, void* stream);
+/* CFG + PNDM (diffusers PNDMScheduler.step_plms with skip_prk_steps; the default scheduler of SD-1.5 pipelines) in the same
+ * graph-replayable form, one launch per step: rows is [num_calls][8] fp32 = (UNet timestep, sample_coeff, eps_coeff, weight
+ * on the new eps, weights on ring slots 1..3, flags: 1 push eps, 2 save the sample, 4 restart from the saved sample);
+ * ring [3][n_half] fp32 holds the three most recent pushed eps (slot 1 first), saved [n_half] fp32 the sample of the first
+ * step.  Reads the step from the low 32 bits of *step_ctr and advances it by 1 before the launch completes. */
+int cl_cfg_plms_step_dev(const float* eps2 /* [2B,...] = [uncond | cond] */, float* latents, float* ring, float* saved,
+                         const float* rows, unsigned long long* step_ctr, int64_t n_half, float guidance, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * LoRA side path (diffusers LoRALinearLayer instances created at models.py:89-97,185,316-323).
