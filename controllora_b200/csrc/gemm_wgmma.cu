@@ -2,17 +2,27 @@
 //
 //   D[M,N] = epilogue( A[M,K] * B[N,K]^T ),  bf16 operands, fp32 accumulation in registers.
 //
-// One CTA per 128 x BN output tile (x one K range under split-K), 288 threads:
+// One CTA per 128 x BN output tile (x one K range under split-K):
 //   warpgroups 0-1 consumers: rows 0-63 / 64-127 of the tile, wgmma.m64n(BN+EXT)k16 straight from the swizzled stages,
-//                  then the epilogue from the accumulator registers (bias, per-image row bias, residual, LoRA, store).
-//   warp 8         TMA producer (one elected thread): A tile 128 x BK, B tile BN x BK [+16 LoRA-down rows],
-//                  128B (BK = 64) or 64B (BK = 32) swizzle, mbarrier ring of up to 8 stages
-// Occupancy OCC = 1 or 2 CTAs per SM is a template parameter: it sets the register cap (224 or 96 per thread; no
-// setmaxnreg, so the producer warp holds as many as a consumer) and the shared memory a launch may use.  With two CTAs on
-// an SM, one CTA's prologue, pipeline fill and register epilogue run while the other's MMAs do, which is what short-K
-// tiles (a few k-blocks each) need; deep-K tiles keep one CTA per SM and the deeper ring.
+//                  then the epilogue from the accumulator registers (bias, per-image row bias, residual, store).
+//   TMA loads (one thread): A tile 128 x BK, B tile BN x BK [+16 LoRA-down rows], 128B (BK = 64) or 64B (BK = 32)
+//                  swizzle, mbarrier ring of up to 8 stages.
+// Occupancy OCC = 1 or 2 CTAs per SM is a template parameter; with two CTAs on an SM, one CTA's prologue, pipeline fill
+// and epilogue run while the other's MMAs do, which is what short-K tiles (a few k-blocks each) need.  Two thread
+// layouts (GemmLayout):
+//   producer warp: 288 threads, the loads come from warp 8, which runs ahead through the whole ring; cap 224 registers
+//                  at one CTA per SM, 96 at two (18 warps put five on one register-file quarter).
+//   no producer:   256 threads, thread 0 of warpgroup 0 fills the ring at tile start and refills each stage once both
+//                  warpgroups have released it; cap 128 at two CTAs per SM.  Used only by the two-CTA tiles that do not
+//                  fit 96 registers (BN 160, LoRA): ptxas serialises their wgmma groups (C7518, the refill is a
+//                  divergent path inside the MMA loop), which they still come out ahead with, and which the 96-register
+//                  tiles avoid by keeping the producer warp.
+// Both layouts issue the same MMA sequence.
 // LoRA (EXT = 16): the 16 extra B rows (bf16 hi / lo halves of the rank-r down matrix) make the main loop produce
-// t = x A^T in 16 extra accumulator columns; the epilogue forms t (+ t_add, -> t_out) and adds scale * t B_up^T in fp32.
+// t = x A^T in 16 extra accumulator columns.  After the main loop, t (+ t_add, -> t_out) is scaled, split exactly into
+// three bf16 parts t1 + t2 + t3 (as is B_up = b1 + b2 + b3) and added to the BN output columns on the tensor cores: three
+// register-A wgmma k16 steps [t1 | t2] * [b1 ; b1] + [t1 | t2] * [b2 ; b2] + [t1 | t3] * [b3 ; b1], which keep every
+// product down to 2^-16 relative; B_up's parts are staged in shared memory in the prologue.
 // The A operand is either a plain row-major matrix or an NHWC image read as 3x3 windows (implicit GEMM: the
 // "im2col" is done by TMA box loads with shifted coordinates, out-of-bounds zero fill == conv zero padding).
 //
@@ -30,16 +40,24 @@
 namespace clb {
 
 static constexpr int BLOCK_M = 128;
-static constexpr int NUM_THREADS = 288;
 static constexpr int PRODUCER_WARP = 8;
+static constexpr int CONSUMER_THREADS = 256;
 // Dynamic shared memory per CTA: 227 KB for one CTA per SM; for two, half of the SM's 228 KB less the 1 KB the hardware
 // reserves per CTA.
 template <int OCC> struct GemmOcc {
     static_assert(OCC == 1 || OCC == 2, "OCC");
     static constexpr int SMEM_LIMIT = OCC == 1 ? 232448 : 115712;
-    // One CTA: 65536 registers / 288 threads, rounded down to 8.  Two CTAs: 18 warps over the SM's four 16384-register
-    // quarters put 5 warps on one quarter, so 16384 / (5 * 32) = 102, rounded down to 8.
-    static constexpr int MAX_REGS = OCC == 1 ? 224 : 96;
+};
+template <int BN, int EXT, int BK, int OCC> struct GemmLayout {
+    // the producer-warp layout unless two CTAs per SM need more than 96 registers (BN 160 or the LoRA tiles)
+    static constexpr bool PRODUCER = OCC == 1 || (EXT == 0 && BN <= 128);
+    static constexpr int NUM_THREADS = PRODUCER ? CONSUMER_THREADS + 32 : CONSUMER_THREADS;
+    // One CTA: 65536 registers / 288 threads, rounded down to 8.  Two CTAs of 288 threads: 18 warps over the SM's four
+    // 16384-register quarters put 5 warps on one, so 16384 / (5 * 32) = 102, rounded down to 8; of 256 threads: 4 warps
+    // on each quarter, 16384 / (4 * 32) = 128.
+    static constexpr int MAX_REGS = OCC == 1 ? 224 : PRODUCER ? 96 : 128;
+    // the thread that initialises the barriers and issues the TMA loads
+    static constexpr int TMA_THREAD = PRODUCER ? PRODUCER_WARP * 32 : 0;
 };
 
 struct GemmParams {
@@ -81,6 +99,9 @@ struct GemmCfg {
     static constexpr int SBO = 8 * ROW_BYTES;                 // 8-row swizzle atom
     static constexpr uint32_t SWZ = (BK == 64) ? SWZ_128B : SWZ_64B;
     static constexpr int ACC = NT / 2;                        // fp32 accumulators per consumer thread
+    // LoRA rank-update B operand (B_up of the tile's BN columns): three k16 steps of BN x 16 bf16, K-major, no swizzle
+    static constexpr int UP_STEP_BYTES = BN * 32;
+    static constexpr int UP_BYTES = EXT ? 3 * UP_STEP_BYTES : 0;
     static_assert(BK == 64 || BK == 32, "BK");
     static_assert(NT % 16 == 0 && NT <= 256, "wgmma N");
     static_assert(BN % 32 == 0, "BN");
@@ -108,15 +129,53 @@ __device__ __forceinline__ void decode_row(const GemmParams& p, int m_blk, int r
     }
 }
 
+// (a, b) -> three bf16x2 parts whose sum is exactly (a, b): each residual is exact in fp32 and 8 + 8 + 8 bits cover
+// fp32's 24-bit significand (short of bf16's underflow range).
+__device__ __forceinline__ void split3_bf16x2(float a, float b, uint32_t& p1, uint32_t& p2, uint32_t& p3) {
+    p1 = pack_bf16x2(a, b);
+    const float2 f1 = unpack_bf16x2(p1);
+    const float ra = a - f1.x, rb = b - f1.y;
+    p2 = pack_bf16x2(ra, rb);
+    const float2 f2 = unpack_bf16x2(p2);
+    p3 = pack_bf16x2(ra - f2.x, rb - f2.y);
+}
+
+// Loads k-block kb of the tile into ring stage `stage` (A tile, B tile and the LoRA-down rows) on its full barrier.
+// Convs: (tw, th, tn) is the tile's position and (tap, cb) = (kb / cblocks, kb % cblocks), which the caller steps along.
+template <int BN, int EXT, int BK>
+__device__ __forceinline__ void load_stage(const CUtensorMap* tmA, const CUtensorMap* tmB, const CUtensorMap* tmE,
+                                           const GemmParams& p, uint8_t* smem, uint64_t* full_bar, int stage, int kb,
+                                           int m_blk, int n_blk, int tw, int th, int tn, int tap, int cb) {
+    using Cfg = GemmCfg<BN, EXT, BK>;
+    mbar_arrive_expect_tx(&full_bar[stage], Cfg::A_BYTES + Cfg::B_BYTES);
+    uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
+    uint8_t* sb = sa + Cfg::A_BYTES;
+    if (p.a_mode == 0) {
+        tma_load_2d(tmA, &full_bar[stage], sa, kb * BK, m_blk * BLOCK_M);
+    } else {
+        const int ky = tap / 3, kx = tap - ky * 3;
+        if (p.a_mode == 1) {
+            tma_load_4d(tmA, &full_bar[stage], sa, cb * BK, tw * p.bw + kx - 1, th * p.bh + ky - 1, tn * p.bn);
+        } else {
+            const int iy = ky - p.pad_lo, ix = kx - p.pad_lo;
+            tma_load_5d(tmA, &full_bar[stage], sa, (ix & 1) * p.C + cb * BK, tw * p.bw + (ix >> 1), iy & 1,
+                        th * p.bh + (iy >> 1), tn * p.bn);
+        }
+    }
+    tma_load_2d(tmB, &full_bar[stage], sb, kb * BK, n_blk * BN);
+    if (EXT) tma_load_2d(tmE, &full_bar[stage], sb + BN * Cfg::ROW_BYTES, kb * BK, 0);
+}
+
 template <int BN, int EXT, int BK, int OCC>
-__global__ void __maxnreg__(GemmOcc<OCC>::MAX_REGS)
+__global__ void __maxnreg__((GemmLayout<BN, EXT, BK, OCC>::MAX_REGS))
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmE, const GemmParams p, const int num_stages) {
     pdl_launch_dependents();
     using Cfg = GemmCfg<BN, EXT, BK>;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + num_stages * Cfg::STAGE_BYTES);
+    uint8_t* s_up = smem + num_stages * Cfg::STAGE_BYTES;
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_up + Cfg::UP_BYTES);
     uint64_t* empty_bar = full_bar + num_stages;
     const int warp_idx = uniform_warp_idx();
     const int lane = threadIdx.x & 31;
@@ -130,7 +189,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const int kb0 = split * p.kb_per_split;
     const int kb1 = min(p.num_k_blocks, kb0 + p.kb_per_split);
 
-    if (warp_idx == PRODUCER_WARP && lane == 0) {
+    using Layout = GemmLayout<BN, EXT, BK, OCC>;
+    int tw = 0, th = 0, tn = 0;   // conv tile position (TMA issue only)
+    if (p.a_mode != 0) {
+        tw = m_blk % p.tiles_w;
+        th = (m_blk / p.tiles_w) % p.tiles_h;
+        tn = m_blk / (p.tiles_w * p.tiles_h);
+    }
+    if (threadIdx.x == Layout::TMA_THREAD) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
         if (EXT) tma_prefetch_desc(&tmE);
@@ -143,42 +209,53 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     __syncthreads();
     pdl_wait();   // everything above touched only shared memory and kernel parameters
 
-    if (warp_idx == PRODUCER_WARP) {
+    if (Layout::PRODUCER && warp_idx == PRODUCER_WARP) {
         if (elect_one_sync()) {
-            int tw = 0, th = 0, tn = 0;
-            if (p.a_mode != 0) {
-                tw = m_blk % p.tiles_w;
-                th = (m_blk / p.tiles_w) % p.tiles_h;
-                tn = m_blk / (p.tiles_w * p.tiles_h);
-            }
             int stage = 0;
             uint32_t phase = 0;
             int tap = 0, cb = 0;
             if (p.a_mode != 0) { tap = kb0 / p.cblocks; cb = kb0 - tap * p.cblocks; }
             for (int kb = kb0; kb < kb1; ++kb) {
                 mbar_wait(&empty_bar[stage], phase ^ 1);
-                mbar_arrive_expect_tx(&full_bar[stage], Cfg::A_BYTES + Cfg::B_BYTES);
-                uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
-                uint8_t* sb = sa + Cfg::A_BYTES;
-                if (p.a_mode == 0) {
-                    tma_load_2d(&tmA, &full_bar[stage], sa, kb * BK, m_blk * BLOCK_M);
-                } else {
-                    const int ky = tap / 3, kx = tap - ky * 3;
-                    if (p.a_mode == 1) {
-                        tma_load_4d(&tmA, &full_bar[stage], sa, cb * BK, tw * p.bw + kx - 1, th * p.bh + ky - 1, tn * p.bn);
-                    } else {
-                        const int iy = ky - p.pad_lo, ix = kx - p.pad_lo;
-                        tma_load_5d(&tmA, &full_bar[stage], sa, (ix & 1) * p.C + cb * BK, tw * p.bw + (ix >> 1), iy & 1,
-                                    th * p.bh + (iy >> 1), tn * p.bn);
-                    }
-                    if (++cb == p.cblocks) { cb = 0; ++tap; }
-                }
-                tma_load_2d(&tmB, &full_bar[stage], sb, kb * BK, n_blk * BN);
-                if (EXT) tma_load_2d(&tmE, &full_bar[stage], sb + BN * Cfg::ROW_BYTES, kb * BK, 0);
+                load_stage<BN, EXT, BK>(&tmA, &tmB, &tmE, p, smem, full_bar, stage, kb, m_blk, n_blk, tw, th, tn, tap, cb);
+                if (p.a_mode != 0 && ++cb == p.cblocks) { cb = 0; ++tap; }
                 if (++stage == num_stages) { stage = 0; phase ^= 1; }
             }
         }
         return;
+    }
+    const bool tma_thread = !Layout::PRODUCER && threadIdx.x == Layout::TMA_THREAD;
+    if (tma_thread) {   // fill the ring; the main loop refills it
+        for (int kb = kb0; kb < kb1 && kb - kb0 < num_stages; ++kb)
+            load_stage<BN, EXT, BK>(&tmA, &tmB, &tmE, p, smem, full_bar, kb - kb0, kb, m_blk, n_blk, tw, th, tn,
+                                    kb / p.cblocks, kb % p.cblocks);
+    }
+
+    if (EXT) {
+        // B operand of the rank update while the ring fills: B_up rows of this tile's columns (zero past N and past the
+        // rank), split into bf16 b1 + b2 + b3.  Core matrices of 8 rows x 16 bytes, (row group g, k half h) at
+        // g * 256 + h * 128; the steps hold k = [b1 | b1], [b2 | b2], [b3 | b1] (k = rank index j in each half).
+        for (int n = threadIdx.x; n < BN; n += CONSUMER_THREADS) {
+            const int gn = n_blk * BN + n;
+            float u[8];
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj)
+                u[jj] = (gn < p.N && jj < p.lora_rp) ? __ldg(p.lora_up + (long long)gn * p.lora_rp + jj) : 0.f;
+            uint4 b1, b2, b3;
+            split3_bf16x2(u[0], u[1], b1.x, b2.x, b3.x);
+            split3_bf16x2(u[2], u[3], b1.y, b2.y, b3.y);
+            split3_bf16x2(u[4], u[5], b1.z, b2.z, b3.z);
+            split3_bf16x2(u[6], u[7], b1.w, b2.w, b3.w);
+            const uint32_t dst = smem_u32(s_up) + (n >> 3) * 256 + (n & 7) * 16;
+            st_shared_u4(dst, b1);
+            st_shared_u4(dst + 128, b1);
+            st_shared_u4(dst + Cfg::UP_STEP_BYTES, b2);
+            st_shared_u4(dst + Cfg::UP_STEP_BYTES + 128, b2);
+            st_shared_u4(dst + 2 * Cfg::UP_STEP_BYTES, b3);
+            st_shared_u4(dst + 2 * Cfg::UP_STEP_BYTES + 128, b1);
+        }
+        fence_proxy_async_smem();                   // generic-proxy stores -> wgmma operand reads
+        named_bar_sync(1, CONSUMER_THREADS);
     }
 
     // ===================================================== consumers: main loop
@@ -188,7 +265,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const uint32_t a_off = uint32_t(wg) * 64 * Cfg::ROW_BYTES;
     {
         int stage = 0, prev = -1;
-        uint32_t phase = 0;
+        uint32_t phase = 0, prev_phase = 0;
         for (int kb = kb0; kb < kb1; ++kb) {
             mbar_wait(&full_bar[stage], phase);
             const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES);
@@ -200,72 +277,66 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                                           make_smem_desc(sb + k * 32, 16, Cfg::SBO, Cfg::SWZ), (kb > kb0 || k > 0) ? 1 : 0);
             wgmma_commit();
             wgmma_wait<1>();          // the previous k-block's MMAs are done: release its stage
-            if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+            if (prev >= 0) {
+                if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+                // no producer warp: once both warpgroups have released it, the stage takes the k-block num_stages on
+                if (tma_thread && kb - 1 + num_stages < kb1) {
+                    mbar_wait(&empty_bar[prev], prev_phase);
+                    const int kn = kb - 1 + num_stages;
+                    load_stage<BN, EXT, BK>(&tmA, &tmB, &tmE, p, smem, full_bar, prev, kn, m_blk, n_blk, tw, th, tn,
+                                            kn / p.cblocks, kn % p.cblocks);
+                }
+            }
             prev = stage;
+            prev_phase = phase;
             if (++stage == num_stages) { stage = 0; phase ^= 1; }
         }
         wgmma_wait<0>();
         wgmma_fence_acc(acc);
     }
 
-    // ===================================================== epilogue from registers
+    // ===================================================== LoRA rank update, then the epilogue from registers
     // accumulator layout of wgmma m64nNk16: acc[j*4 + i*2 + c] = D[row w*16 + lane/4 + 8i][col 8j + 2*(lane%4) + c]
     const int w4 = warp_idx & 3, q = lane & 3;
-    // Both rows of this lane first (row index, row_bias group, LoRA t), then the columns: each column's lora_up values are
-    // loaded once for the two rows.
     int m[2], grp[2];
-    float t[2][8];
 #pragma unroll
-    for (int i = 0; i < 2; ++i) {
-        decode_row(p, m_blk, wg * 64 + w4 * 16 + (lane >> 2) + 8 * i, m[i], grp[i]);
-        if (EXT) {
-            // t[j] = e[j] + e[j + 8]: this lane holds columns 2q, 2q+1 of both halves; gather the quad's 8 values
-            const float t0 = acc[(BN / 8) * 4 + i * 2] + acc[(BN / 8 + 1) * 4 + i * 2];
-            const float t1 = acc[(BN / 8) * 4 + i * 2 + 1] + acc[(BN / 8 + 1) * 4 + i * 2 + 1];
+    for (int i = 0; i < 2; ++i) decode_row(p, m_blk, wg * 64 + w4 * 16 + (lane >> 2) + 8 * i, m[i], grp[i]);
+    if constexpr (EXT != 0) {
+        // t[j] = e[j] + e[j + 8]: this lane holds t columns 2q, 2q+1 of rows i = 0, 1, which is where the register-A
+        // fragment of a k16 step wants k = 2q, 2q+1 (a0 / a1) and k = 8 + 2q, 9 + 2q (a2 / a3).
+        const int rp = p.lora_rp;
+        uint32_t tp1[2], tp2[2], tp3[2];   // s t = tp1 + tp2 + tp3
 #pragma unroll
-            for (int qq = 0; qq < 4; ++qq) {
-                t[i][2 * qq] = __shfl_sync(0xffffffffu, t0, (lane & ~3) | qq);
-                t[i][2 * qq + 1] = __shfl_sync(0xffffffffu, t1, (lane & ~3) | qq);
-            }
-            const int rp = p.lora_rp;
-            if (m[i] >= 0) {
+        for (int i = 0; i < 2; ++i) {
+            float t0 = acc[(BN / 8) * 4 + i * 2] + acc[(BN / 8 + 1) * 4 + i * 2];
+            float t1 = acc[(BN / 8) * 4 + i * 2 + 1] + acc[(BN / 8 + 1) * 4 + i * 2 + 1];
+            if (m[i] >= 0 && 2 * q < rp) {   // rp is even
                 const long long tb = (long long)m[i] * rp;
-                float o0 = t0, o1 = t1;   // this lane's own columns 2q, 2q+1, so t is never indexed by the lane
-                if (p.t_add != nullptr) {
-                    if (2 * q < rp) { o0 += p.t_add[tb + 2 * q]; o1 += p.t_add[tb + 2 * q + 1]; }   // rp is even
-#pragma unroll
-                    for (int jj = 0; jj < 8; ++jj)
-                        if (jj < rp) t[i][jj] += p.t_add[tb + jj];
-                }
-                if (p.t_out != nullptr && n_blk == 0 && 2 * q < rp) { p.t_out[tb + 2 * q] = o0; p.t_out[tb + 2 * q + 1] = o1; }
+                if (p.t_add != nullptr) { t0 += p.t_add[tb + 2 * q]; t1 += p.t_add[tb + 2 * q + 1]; }
+                if (p.t_out != nullptr && n_blk == 0) { p.t_out[tb + 2 * q] = t0; p.t_out[tb + 2 * q + 1] = t1; }
             }
-#pragma unroll
-            for (int jj = 0; jj < 8; ++jj) t[i][jj] = (jj < rp) ? t[i][jj] * p.lora_scale : 0.f;
+            const float s0 = 2 * q < rp ? t0 * p.lora_scale : 0.f, s1 = 2 * q < rp ? t1 * p.lora_scale : 0.f;
+            split3_bf16x2(s0, s1, tp1[i], tp2[i], tp3[i]);
         }
+        const uint32_t a12[4] = {tp1[0], tp1[1], tp2[0], tp2[1]};
+        const uint32_t a13[4] = {tp1[0], tp1[1], tp3[0], tp3[1]};
+        const uint32_t su = smem_u32(s_up);
+        wgmma_fence();
+        WgmmaRs<BN, 0>::mma(acc, a12, make_smem_desc(su, 128, 256, 0), 1);
+        WgmmaRs<BN, 0>::mma(acc, a12, make_smem_desc(su + Cfg::UP_STEP_BYTES, 128, 256, 0), 1);
+        WgmmaRs<BN, 0>::mma(acc, a13, make_smem_desc(su + 2 * Cfg::UP_STEP_BYTES, 128, 256, 0), 1);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_acc(acc);
     }
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j) {
         const int n = n_blk * BN + 8 * j + 2 * q;
         if (n >= p.N) continue;          // N % 4 == 0: n < N implies n + 1 < N
-        float u0[8], u1[8];
-        if (EXT) {
-            const float* up = p.lora_up + (long long)n * p.lora_rp;
-#pragma unroll
-            for (int jj = 0; jj < 8; ++jj) {
-                u0[jj] = jj < p.lora_rp ? __ldg(up + jj) : 0.f;
-                u1[jj] = jj < p.lora_rp ? __ldg(up + p.lora_rp + jj) : 0.f;
-            }
-        }
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
             if (m[i] < 0) continue;
             float v0 = acc[j * 4 + i * 2], v1 = acc[j * 4 + i * 2 + 1];
-            if (EXT) {
-#pragma unroll
-                for (int jj = 0; jj < 8; ++jj) {
-                    if (jj < p.lora_rp) { v0 = fmaf(t[i][jj], u0[jj], v0); v1 = fmaf(t[i][jj], u1[jj], v1); }
-                }
-            }
             if (p.splits > 1) {     // host cleared bias / row_bias / residual: the finishing kernel applies them
                 *reinterpret_cast<float2*>(p.split_ws + (long long)split * p.M * p.N + (long long)m[i] * p.N + n) = make_float2(v0, v1);
                 continue;
@@ -343,7 +414,8 @@ static int launch_gemm(const CUtensorMap& tA, const CUtensorMap& tB, const CUten
     using Cfg = GemmCfg<BN, EXT, BK>;
     constexpr int SMEM_LIMIT = GemmOcc<OCC>::SMEM_LIMIT;
     GemmParams p = p_in;
-    const int fixed = 1024 /*align slack*/ + 256 /*barriers*/;
+    constexpr int NUM_THREADS = GemmLayout<BN, EXT, BK, OCC>::NUM_THREADS;
+    const int fixed = 1024 /*align slack*/ + Cfg::UP_BYTES + 256 /*barriers*/;
     int stages = (SMEM_LIMIT - fixed) / Cfg::STAGE_BYTES;
     if (stages > 8) stages = 8;
     if (stages < 2) return set_error(CL_ERR_UNSUPPORTED, "cl_gemm: not enough shared memory for 2 stages");
@@ -388,7 +460,10 @@ struct TilePlan { int bn, splits, occ; };
 static inline int gemm_block_k(const cl_gemm_args* a) { return (a->a_mode != 0 && a->C % 64 != 0) ? 32 : 64; }
 
 // The instantiations that compile within GemmOcc<2>::MAX_REGS registers without spilling.
-static inline bool gemm_fits_two_ctas(int bn, bool lora, int BK) { return !lora && (BK == 32 ? bn <= 128 : bn == 128); }
+static inline bool gemm_fits_two_ctas(int bn, bool lora, int BK) {
+    if (BK == 32) return !lora && bn <= 128;
+    return lora ? (bn == 64 || bn == 128 || bn == 160) : (bn == 128 || bn == 160);
+}
 
 static TilePlan plan_tiles(const cl_gemm_args* a, int BK, int num_m_blocks, bool allow_split) {
     const bool lora = a->lora_up != nullptr;
@@ -429,6 +504,8 @@ static TilePlan plan_tiles(const cl_gemm_args* a, int BK, int num_m_blocks, bool
     // CTA slots: then one CTA's prologue, pipeline fill and epilogue overlap the other's MMAs.  Measured on the bench step
     // (H100 SXM): the 9-18 k-block launches with >= 1024 tiles ran 0.79-0.85x the one-CTA time at BK 64 and BN 128;
     // launches of 80-240 tiles were slower at two CTAs per SM (pairs share SMs while others idle), deep-K ones were too.
+    // At BN 160 the 5-20 k-block launches of 384-1536 tiles ran 0.72-0.97x (plain) of their one-CTA step time, and the
+    // LoRA ones 0.57-0.91x (together with the rank update moving onto the tensor cores).
     if (best.splits == 1 && nkb <= 20 && gemm_fits_two_ctas(best.bn, lora, BK)) {
         const long long tiles = (long long)num_m_blocks * ((a->N + best.bn - 1) / best.bn);
         if (tiles >= 2LL * sms) best.occ = 2;
@@ -455,16 +532,16 @@ static int dispatch_gemm(const CUtensorMap& tA, const CUtensorMap& tB, const CUt
     }
     if (lora) {
         switch (bn_sel) {
-            case 64: return launch_gemm<64, 16, 64, 1>(tA, tB, tE, p, stream, q);
-            case 128: return launch_gemm<128, 16, 64, 1>(tA, tB, tE, p, stream, q);
-            case 160: return launch_gemm<160, 16, 64, 1>(tA, tB, tE, p, stream, q);
+            case 64: return two ? launch_gemm<64, 16, 64, 2>(tA, tB, tE, p, stream, q) : launch_gemm<64, 16, 64, 1>(tA, tB, tE, p, stream, q);
+            case 128: return two ? launch_gemm<128, 16, 64, 2>(tA, tB, tE, p, stream, q) : launch_gemm<128, 16, 64, 1>(tA, tB, tE, p, stream, q);
+            case 160: return two ? launch_gemm<160, 16, 64, 2>(tA, tB, tE, p, stream, q) : launch_gemm<160, 16, 64, 1>(tA, tB, tE, p, stream, q);
             default: return set_error(CL_ERR_UNSUPPORTED, "cl_gemm: block_n for LoRA must be 64/128/160");
         }
     }
     switch (bn_sel) {
         case 64: return launch_gemm<64, 0, 64, 1>(tA, tB, tE, p, stream, q);
         case 128: return two ? launch_gemm<128, 0, 64, 2>(tA, tB, tE, p, stream, q) : launch_gemm<128, 0, 64, 1>(tA, tB, tE, p, stream, q);
-        case 160: return launch_gemm<160, 0, 64, 1>(tA, tB, tE, p, stream, q);
+        case 160: return two ? launch_gemm<160, 0, 64, 2>(tA, tB, tE, p, stream, q) : launch_gemm<160, 0, 64, 1>(tA, tB, tE, p, stream, q);
         case 256: return launch_gemm<256, 0, 64, 1>(tA, tB, tE, p, stream, q);
         default: return set_error(CL_ERR_UNSUPPORTED, "cl_gemm: block_n must be 64/128/160/256");
     }
