@@ -822,8 +822,8 @@ def test_adamw_host_step_matches_emulator():
     assert_f32_close(v, ve, "adamw v vs emulator", 1e-6, ve.abs().amax().expand(1))
 
 
-# ------------------------------------------------------------------------------------------------------------ kernels with their own fp64 tests:
-# kernel vs emulator only
+# ------------------------------------------------------------------------------------------------------------ GEMM, attention, norms:
+# kernel vs emulator only here; their per-element fp64 contracts are in tests/test_core_kernel_contracts.py
 def _max_floor(e, rel=2.0**-12):
     return e.detach().abs().float().amax().to(F64).reshape(1) * rel
 
