@@ -4,7 +4,8 @@
 //
 // One CTA per 128 x BN output tile (x one K range under split-K):
 //   warpgroups 0-1 consumers: rows 0-63 / 64-127 of the tile, wgmma.m64n(BN+EXT)k16 straight from the swizzled stages,
-//                  then the epilogue from the accumulator registers (bias, per-image row bias, residual, store).
+//                  then the epilogue: bias, per-image row bias and residual added to the accumulators, the tile staged
+//                  in the drained ring and written by TMA stores (epilogue_tma).
 //   TMA loads (one thread): A tile 128 x BK, B tile BN x BK [+16 LoRA-down rows], 128B (BK = 64) or 64B (BK = 32)
 //                  swizzle, mbarrier ring of up to 8 stages.
 // Occupancy OCC = 1 or 2 CTAs per SM is a template parameter; with two CTAs on an SM, one CTA's prologue, pipeline fill
@@ -14,9 +15,10 @@
 //                  at one CTA per SM, 96 at two (18 warps put five on one register-file quarter).
 //   no producer:   256 threads, thread 0 of warpgroup 0 fills the ring at tile start and refills each stage once both
 //                  warpgroups have released it; cap 128 at two CTAs per SM.  Used only by the two-CTA tiles that do not
-//                  fit 96 registers (BN 160, LoRA): ptxas serialises their wgmma groups (C7518, the refill is a
-//                  divergent path inside the MMA loop), which they still come out ahead with, and which the 96-register
-//                  tiles avoid by keeping the producer warp.
+//                  fit 96 registers (BN 160, LoRA).  Each warpgroup retires a k-block's four MMAs (one commit group)
+//                  before it releases the stage and thread 0 refills it: a single-thread path run while a group is in
+//                  flight makes ptxas serialise every wgmma of the kernel (C7518).  The other CTA on the SM keeps the
+//                  tensor cores busy across that drain.
 // Both layouts issue the same MMA sequence.
 // LoRA (EXT = 16): the 16 extra B rows (bf16 hi / lo halves of the rank-r down matrix) make the main loop produce
 // t = x A^T in 16 extra accumulator columns.  After the main loop, t (+ t_add, -> t_out) is scaled, split exactly into
@@ -83,6 +85,9 @@ struct GemmParams {
     void* out;
     long long ldd;
     int out_fp32;
+    // 1: the output tile (or split-K partial) is staged in shared memory and written by TMA stores (tmD), the residual
+    // read by TMA (tmR)
+    int tma_epilogue;
     // split-K: tile space is (m, n, split); split s covers k-blocks [s*kb_per_split, ...) and stores its fp32 partial tile
     // to split_ws[s][M][N]; splitk_finish_kernel sums the partials and applies the epilogue.
     int splits, kb_per_split;
@@ -166,10 +171,118 @@ __device__ __forceinline__ void load_stage(const CUtensorMap* tmA, const CUtenso
     if (EXT) tma_load_2d(tmE, &full_bar[stage], sb + BN * Cfg::ROW_BYTES, kb * BK, 0);
 }
 
+// TMA epilogue: the output tile is staged in the drained ring as 64-byte-wide column chunks of 128 rows (bf16: 32 columns,
+// fp32: 16), 64B-swizzled like the boxes of tmD / tmR, so that a warp's 8 rows x 16 bytes of one accumulator column pair
+// fall into 32 different banks.  Byte (row, c) sits at chunk c / 64, row * 64, 16-byte unit ((c / 16) % 4) ^ ((row / 2) % 4).
+// The residual tile (bf16 output only) comes in by TMA into the staging chunks; the consumers add bias, row bias and
+// residual to their accumulators in the register epilogue's order and overwrite their own slots; the chunks leave by TMA
+// stores, whose bounds drop rows past M (or past the images) and columns past N.  One thread issues the TMA operations:
+// a producer-warp lane, which holds no accumulators, or thread 0 where there is no producer warp.  Named barrier 2: every
+// MMA has read the ring (and s_up); barrier 3: the staged tile is complete.
+__device__ __forceinline__ void epi_conv_pos(const GemmParams& p, int m_blk, int& x, int& y, int& z) {
+    x = m_blk % p.tiles_w * p.bw;
+    y = (m_blk / p.tiles_w) % p.tiles_h * p.bh;
+    z = m_blk / (p.tiles_w * p.tiles_h) * p.bn;
+}
+
+template <int BN>
+__device__ __forceinline__ void epi_load_residual(const CUtensorMap* tmR, const GemmParams& p, uint8_t* stile,
+                                                  uint64_t* res_bar, int m_blk, int n_blk) {
+    mbar_arrive_expect_tx(res_bar, BLOCK_M * BN * 2);
+    int x = 0, y = 0, z = 0;
+    if (p.a_mode != 0) epi_conv_pos(p, m_blk, x, y, z);
+#pragma unroll 1
+    for (int k = 0; k < BN / 32; ++k) {
+        uint8_t* dst = stile + k * BLOCK_M * 64;
+        if (p.a_mode == 0) tma_load_2d(tmR, res_bar, dst, n_blk * BN + 32 * k, m_blk * BLOCK_M);
+        else tma_load_4d(tmR, res_bar, dst, n_blk * BN + 32 * k, x, y, z);
+    }
+}
+
+// split-K partials go to split_ws[split] through a map with the split as its outermost dimension
+template <int BN>
+__device__ __forceinline__ void epi_store(const CUtensorMap* tmD, const GemmParams& p, uint8_t* stile, int m_blk, int n_blk,
+                                          int split) {
+    const int esz = (p.out_fp32 || p.splits > 1) ? 4 : 2;
+    int x = 0, y = 0, z = 0;
+    if (p.a_mode != 0) epi_conv_pos(p, m_blk, x, y, z);
+    const uint32_t base = smem_u32(stile);
+#pragma unroll 1
+    for (int k = 0; k < BN * esz / 64; ++k) {
+        const int c0 = n_blk * BN * esz / 2 + 32 * k;   // the maps count 2-byte elements
+        const uint32_t src = base + k * BLOCK_M * 64;
+        if (p.splits > 1) {
+            if (p.a_mode == 0) tma_store_3d(tmD, src, c0, m_blk * BLOCK_M, split);
+            else tma_store_5d(tmD, src, c0, x, y, z, split);
+        } else {
+            if (p.a_mode == 0) tma_store_2d(tmD, src, c0, m_blk * BLOCK_M);
+            else tma_store_4d(tmD, src, c0, x, y, z);
+        }
+    }
+    bulk_commit_group();
+    bulk_wait_group_read<0>();             // shared memory stays valid until the stores have read it
+}
+
+// the consumers' half; ISSUE: this kernel has no producer warp, so thread 0 issues the TMA operations
+template <int BN, int ESZ, bool ISSUE, int NACC>
+__device__ __forceinline__ void epilogue_tma(const CUtensorMap* tmD, const CUtensorMap* tmR, const GemmParams& p,
+                                             const float (&acc)[NACC], uint8_t* stile, uint64_t* res_bar, int m_blk,
+                                             int n_blk, int split, const float* const (&rbp)[2], int row0, int q,
+                                             int bar_threads) {
+    const bool res = p.residual != nullptr;
+    named_bar_sync(2, bar_threads);
+    if (res) {
+        if (ISSUE && threadIdx.x == 0) epi_load_residual<BN>(tmR, p, stile, res_bar, m_blk, n_blk);
+        mbar_wait(res_bar, 0);
+    }
+    // this thread's byte columns are 8 j ESZ + 2 q ESZ: the q part, the row's swizzle and the row go into one address per
+    // row, the j part is a constant unit XOR and chunk offset (no carries: 2 q ESZ stays within its 16- or 32-byte group)
+    const uint32_t base = smem_u32(stile);
+    uint32_t addr[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        const int row = row0 + 8 * i, cq = 2 * q * ESZ;
+        addr[i] = base + row * 64 + ((((cq >> 4) ^ (row >> 1)) & 3) << 4) + (cq & 15);
+    }
+    const int n0 = n_blk * BN + 2 * q, n_left = p.N - n0;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+        const int n = n0 + 8 * j;
+        const bool n_in = 8 * j < n_left;  // N % 4 == 0: n < N implies n + 1 < N
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            float v0 = acc[j * 4 + i * 2], v1 = acc[j * 4 + i * 2 + 1];
+            if (p.bias != nullptr && n_in) { v0 += __ldg(p.bias + n); v1 += __ldg(p.bias + n + 1); }
+            if (rbp[i] != nullptr && n_in) {
+                const float2 rb = *reinterpret_cast<const float2*>(rbp[i] + n);
+                v0 += rb.x; v1 += rb.y;
+            }
+            const uint32_t a = (addr[i] ^ ((((8 * j * ESZ) >> 4) & 3) << 4)) + ((8 * j * ESZ) >> 6) * (BLOCK_M * 64);
+            if (ESZ == 4) {
+                st_shared_f2(a, v0, v1);
+            } else {
+                if (res) {
+                    const float2 rr = unpack_bf16x2(ld_shared_u32(a));
+                    v0 += rr.x; v1 += rr.y;
+                }
+                st_shared_u32(a, pack_bf16x2(v0, v1));
+            }
+        }
+    }
+    fence_proxy_async_smem();              // generic-proxy stores -> TMA reads
+    if (ISSUE) {
+        named_bar_sync(3, bar_threads);
+        if (threadIdx.x == 0) epi_store<BN>(tmD, p, stile, m_blk, n_blk, split);
+    } else {
+        named_bar_arrive(3, bar_threads);
+    }
+}
+
 template <int BN, int EXT, int BK, int OCC>
 __global__ void __maxnreg__((GemmLayout<BN, EXT, BK, OCC>::MAX_REGS))
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                  const __grid_constant__ CUtensorMap tmE, const GemmParams p, const int num_stages) {
+                  const __grid_constant__ CUtensorMap tmE, const __grid_constant__ CUtensorMap tmD,
+                  const __grid_constant__ CUtensorMap tmR, const GemmParams p, const int num_stages) {
     pdl_launch_dependents();
     using Cfg = GemmCfg<BN, EXT, BK>;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -177,6 +290,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     uint8_t* s_up = smem + num_stages * Cfg::STAGE_BYTES;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_up + Cfg::UP_BYTES);
     uint64_t* empty_bar = full_bar + num_stages;
+    uint64_t* res_bar = empty_bar + num_stages;    // residual tile of the TMA epilogue
     const int warp_idx = uniform_warp_idx();
     const int lane = threadIdx.x & 31;
     const int wg = warp_idx >> 2;
@@ -204,6 +318,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             mbar_init(&full_bar[i], 1);
             mbar_init(&empty_bar[i], 2);     // one arrival per consumer warpgroup
         }
+        mbar_init(res_bar, 1);
         fence_barrier_init();
     }
     __syncthreads();
@@ -221,6 +336,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 if (p.a_mode != 0 && ++cb == p.cblocks) { cb = 0; ++tap; }
                 if (++stage == num_stages) { stage = 0; phase ^= 1; }
             }
+        }
+        __syncwarp();
+        if (p.tma_epilogue) {   // the TMA epilogue's loads and stores, issued for the consumers
+            named_bar_sync(2, Layout::NUM_THREADS);
+            if (lane == 0 && p.residual != nullptr) epi_load_residual<BN>(&tmR, p, smem, res_bar, m_blk, n_blk);
+            named_bar_sync(3, Layout::NUM_THREADS);
+            if (lane == 0) epi_store<BN>(&tmD, p, smem, m_blk, n_blk, split);
         }
         return;
     }
@@ -265,7 +387,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const uint32_t a_off = uint32_t(wg) * 64 * Cfg::ROW_BYTES;
     {
         int stage = 0, prev = -1;
-        uint32_t phase = 0, prev_phase = 0;
+        uint32_t phase = 0;
         for (int kb = kb0; kb < kb1; ++kb) {
             mbar_wait(&full_bar[stage], phase);
             const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES);
@@ -276,26 +398,31 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 Wgmma<Cfg::NT, 0, 0>::mma(acc, make_smem_desc(sa + a_off + k * 32, 16, Cfg::SBO, Cfg::SWZ),
                                           make_smem_desc(sb + k * 32, 16, Cfg::SBO, Cfg::SWZ), (kb > kb0 || k > 0) ? 1 : 0);
             wgmma_commit();
-            wgmma_wait<1>();          // the previous k-block's MMAs are done: release its stage
-            if (prev >= 0) {
-                if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
-                // no producer warp: once both warpgroups have released it, the stage takes the k-block num_stages on
-                if (tma_thread && kb - 1 + num_stages < kb1) {
-                    mbar_wait(&empty_bar[prev], prev_phase);
-                    const int kn = kb - 1 + num_stages;
-                    load_stage<BN, EXT, BK>(&tmA, &tmB, &tmE, p, smem, full_bar, prev, kn, m_blk, n_blk, tw, th, tn,
+            if constexpr (Layout::PRODUCER) {
+                wgmma_wait<1>();      // the previous k-block's MMAs are done: release its stage
+                if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+                prev = stage;
+            } else {
+                // No producer warp: the release and the refill are single-thread paths, which ptxas answers by
+                // serialising every wgmma of the kernel when they run with a group in flight.  So this k-block's group
+                // retires first, and the other CTA on the SM keeps the tensor cores busy across the drain.
+                wgmma_wait<0>();
+                if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[stage]);
+                // once both warpgroups have released it, the stage takes the k-block num_stages on
+                if (tma_thread && kb + num_stages < kb1) {
+                    mbar_wait(&empty_bar[stage], phase);
+                    const int kn = kb + num_stages;
+                    load_stage<BN, EXT, BK>(&tmA, &tmB, &tmE, p, smem, full_bar, stage, kn, m_blk, n_blk, tw, th, tn,
                                             kn / p.cblocks, kn % p.cblocks);
                 }
             }
-            prev = stage;
-            prev_phase = phase;
             if (++stage == num_stages) { stage = 0; phase ^= 1; }
         }
         wgmma_wait<0>();
         wgmma_fence_acc(acc);
     }
 
-    // ===================================================== LoRA rank update, then the epilogue from registers
+    // ===================================================== LoRA rank update, then the epilogue
     // accumulator layout of wgmma m64nNk16: acc[j*4 + i*2 + c] = D[row w*16 + lane/4 + 8i][col 8j + 2*(lane%4) + c]
     const int w4 = warp_idx & 3, q = lane & 3;
     int m[2], grp[2];
@@ -329,6 +456,21 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         wgmma_wait<0>();
         wgmma_fence_acc(acc);
     }
+    if (p.tma_epilogue) {
+        const int row0 = wg * 64 + w4 * 16 + (lane >> 2);
+        // row bias of each of this thread's two rows (none past M or past the images)
+        const float* rbp[2];
+#pragma unroll
+        for (int i = 0; i < 2; ++i) rbp[i] = (p.row_bias != nullptr && m[i] >= 0) ? p.row_bias + (long long)grp[i] * p.ld_rb : nullptr;
+        constexpr bool ISSUE = !Layout::PRODUCER;
+        if (p.out_fp32 || p.splits > 1)   // split-K partials are fp32, with no epilogue inputs (the finishing kernel adds them)
+            epilogue_tma<BN, 4, ISSUE>(&tmD, &tmR, p, acc, smem, res_bar, m_blk, n_blk, split, rbp, row0, q, Layout::NUM_THREADS);
+        else
+            epilogue_tma<BN, 2, ISSUE>(&tmD, &tmR, p, acc, smem, res_bar, m_blk, n_blk, split, rbp, row0, q, Layout::NUM_THREADS);
+        return;
+    }
+    // register epilogue: outputs, residuals or split-K workspaces a TMA map cannot address (not 16-byte aligned), fp32
+    // outputs with a residual
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j) {
         const int n = n_blk * BN + 8 * j + 2 * q;
@@ -409,8 +551,8 @@ splitk_finish_kernel(const float* __restrict__ ws, int splits, int M, int N, con
 // Launches the GEMM; with `resident` set, launches nothing and stores how many CTAs of this instantiation the device keeps
 // resident per SM at the shared-memory size the launch would use.
 template <int BN, int EXT, int BK, int OCC>
-static int launch_gemm(const CUtensorMap& tA, const CUtensorMap& tB, const CUtensorMap& tE, const GemmParams& p_in,
-                       cudaStream_t stream, int* resident) {
+static int launch_gemm(const CUtensorMap& tA, const CUtensorMap& tB, const CUtensorMap& tE, const CUtensorMap& tD,
+                       const CUtensorMap& tR, const GemmParams& p_in, cudaStream_t stream, int* resident) {
     using Cfg = GemmCfg<BN, EXT, BK>;
     constexpr int SMEM_LIMIT = GemmOcc<OCC>::SMEM_LIMIT;
     GemmParams p = p_in;
@@ -422,6 +564,9 @@ static int launch_gemm(const CUtensorMap& tA, const CUtensorMap& tB, const CUten
     const int smem_bytes = fixed + stages * Cfg::STAGE_BYTES;
     const long long grid = (long long)p.num_m_blocks * p.num_n_blocks * p.splits;
     if (grid > 0x7fffffffLL) return set_error(CL_ERR_UNSUPPORTED, "cl_gemm: too many tiles");
+    // the staged output tile has to fit the ring (and s_up behind it)
+    if ((long long)BLOCK_M * BN * ((p.out_fp32 || p.splits > 1) ? 4 : 2) > (long long)stages * Cfg::STAGE_BYTES + Cfg::UP_BYTES)
+        p.tma_epilogue = 0;
     const GemmParams full = p;
     if (p.splits > 1) { p.bias = nullptr; p.row_bias = nullptr; p.residual = nullptr; }
     static bool attr_done = false;
@@ -433,7 +578,8 @@ static int launch_gemm(const CUtensorMap& tA, const CUtensorMap& tB, const CUten
         CL_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(resident, gemm_wgmma_kernel<BN, EXT, BK, OCC>, NUM_THREADS, smem_bytes));
         return CL_OK;
     }
-    launch_k_pdl(gemm_wgmma_kernel<BN, EXT, BK, OCC>, (unsigned)grid, NUM_THREADS, smem_bytes, stream, tA, tB, tE, p, stages);
+    launch_k_pdl(gemm_wgmma_kernel<BN, EXT, BK, OCC>, (unsigned)grid, NUM_THREADS, smem_bytes, stream, tA, tB, tE, tD, tR, p,
+                 stages);
     count_launch();
     if (p.splits > 1) {
         const long long quads = (long long)p.M * (p.N / 4);
@@ -519,30 +665,31 @@ extern "C" int cl_gemm_split_hint(const cl_gemm_args* a) {
     return plan_tiles(a, gemm_block_k(a), (a->M + BLOCK_M - 1) / BLOCK_M, true).splits;
 }
 
-static int dispatch_gemm(const CUtensorMap& tA, const CUtensorMap& tB, const CUtensorMap& tE, const GemmParams& p,
-                         cudaStream_t stream, int* q, int bn_sel, bool two, bool lora, int BK) {
+static int dispatch_gemm(const CUtensorMap& tA, const CUtensorMap& tB, const CUtensorMap& tE, const CUtensorMap& tD,
+                         const CUtensorMap& tR, const GemmParams& p, cudaStream_t stream, int* q, int bn_sel, bool two,
+                         bool lora, int BK) {
     if (BK == 32) {
         if (lora) return set_error(CL_ERR_UNSUPPORTED, "cl_gemm: LoRA epilogue is not instantiated for 32-channel convs");
         switch (bn_sel) {
-            case 32: return two ? launch_gemm<32, 0, 32, 2>(tA, tB, tE, p, stream, q) : launch_gemm<32, 0, 32, 1>(tA, tB, tE, p, stream, q);
-            case 64: return two ? launch_gemm<64, 0, 32, 2>(tA, tB, tE, p, stream, q) : launch_gemm<64, 0, 32, 1>(tA, tB, tE, p, stream, q);
-            case 128: return two ? launch_gemm<128, 0, 32, 2>(tA, tB, tE, p, stream, q) : launch_gemm<128, 0, 32, 1>(tA, tB, tE, p, stream, q);
+            case 32: return two ? launch_gemm<32, 0, 32, 2>(tA, tB, tE, tD, tR, p, stream, q) : launch_gemm<32, 0, 32, 1>(tA, tB, tE, tD, tR, p, stream, q);
+            case 64: return two ? launch_gemm<64, 0, 32, 2>(tA, tB, tE, tD, tR, p, stream, q) : launch_gemm<64, 0, 32, 1>(tA, tB, tE, tD, tR, p, stream, q);
+            case 128: return two ? launch_gemm<128, 0, 32, 2>(tA, tB, tE, tD, tR, p, stream, q) : launch_gemm<128, 0, 32, 1>(tA, tB, tE, tD, tR, p, stream, q);
             default: return set_error(CL_ERR_UNSUPPORTED, "cl_gemm: block_n for 32-channel convs must be 32/64/128");
         }
     }
     if (lora) {
         switch (bn_sel) {
-            case 64: return two ? launch_gemm<64, 16, 64, 2>(tA, tB, tE, p, stream, q) : launch_gemm<64, 16, 64, 1>(tA, tB, tE, p, stream, q);
-            case 128: return two ? launch_gemm<128, 16, 64, 2>(tA, tB, tE, p, stream, q) : launch_gemm<128, 16, 64, 1>(tA, tB, tE, p, stream, q);
-            case 160: return two ? launch_gemm<160, 16, 64, 2>(tA, tB, tE, p, stream, q) : launch_gemm<160, 16, 64, 1>(tA, tB, tE, p, stream, q);
+            case 64: return two ? launch_gemm<64, 16, 64, 2>(tA, tB, tE, tD, tR, p, stream, q) : launch_gemm<64, 16, 64, 1>(tA, tB, tE, tD, tR, p, stream, q);
+            case 128: return two ? launch_gemm<128, 16, 64, 2>(tA, tB, tE, tD, tR, p, stream, q) : launch_gemm<128, 16, 64, 1>(tA, tB, tE, tD, tR, p, stream, q);
+            case 160: return two ? launch_gemm<160, 16, 64, 2>(tA, tB, tE, tD, tR, p, stream, q) : launch_gemm<160, 16, 64, 1>(tA, tB, tE, tD, tR, p, stream, q);
             default: return set_error(CL_ERR_UNSUPPORTED, "cl_gemm: block_n for LoRA must be 64/128/160");
         }
     }
     switch (bn_sel) {
-        case 64: return launch_gemm<64, 0, 64, 1>(tA, tB, tE, p, stream, q);
-        case 128: return two ? launch_gemm<128, 0, 64, 2>(tA, tB, tE, p, stream, q) : launch_gemm<128, 0, 64, 1>(tA, tB, tE, p, stream, q);
-        case 160: return two ? launch_gemm<160, 0, 64, 2>(tA, tB, tE, p, stream, q) : launch_gemm<160, 0, 64, 1>(tA, tB, tE, p, stream, q);
-        case 256: return launch_gemm<256, 0, 64, 1>(tA, tB, tE, p, stream, q);
+        case 64: return launch_gemm<64, 0, 64, 1>(tA, tB, tE, tD, tR, p, stream, q);
+        case 128: return two ? launch_gemm<128, 0, 64, 2>(tA, tB, tE, tD, tR, p, stream, q) : launch_gemm<128, 0, 64, 1>(tA, tB, tE, tD, tR, p, stream, q);
+        case 160: return two ? launch_gemm<160, 0, 64, 2>(tA, tB, tE, tD, tR, p, stream, q) : launch_gemm<160, 0, 64, 1>(tA, tB, tE, tD, tR, p, stream, q);
+        case 256: return launch_gemm<256, 0, 64, 1>(tA, tB, tE, tD, tR, p, stream, q);
         default: return set_error(CL_ERR_UNSUPPORTED, "cl_gemm: block_n must be 64/128/160/256");
     }
 }
@@ -653,10 +800,47 @@ static int run_gemm(const cl_gemm_args* a, cudaStream_t stream, int32_t* info) {
     if (p.row_bias && p.rows_per_group <= 0) return set_error(CL_ERR_INVALID, "cl_gemm: rows_per_group");
     if ((p.ldd % 4) || (p.residual && (p.ldr % 4))) return set_error(CL_ERR_INVALID, "cl_gemm: ldd/ldr % 4");
 
+    // TMA epilogue: output (and residual) as 2-D maps, or for convs 4-D maps over the output image, in 64-byte column boxes
+    // of 128 rows (the conv tile's bw x bh x bn box); an fp32 output is addressed as pairs of 2-byte elements.  Split-K
+    // partials: the same over split_ws ([splits][M][N] fp32) with the split as one more, outermost dimension.
+    CUtensorMap tD, tR;
+    memset(&tD, 0, sizeof(tD));
+    memset(&tR, 0, sizeof(tR));
+    const bool split = p.splits > 1;
+    const int esz = (p.out_fp32 || split) ? 4 : 2;
+    void* const dst = split ? static_cast<void*>(p.split_ws) : p.out;
+    const uint64_t ldd = (split ? (uint64_t)p.N : (uint64_t)p.ldd) * esz, ldr = p.ldr * 2;
+    const bool res = !split && p.residual != nullptr;
+    p.tma_epilogue = (reinterpret_cast<uintptr_t>(dst) & 15) == 0 && ldd % 16 == 0 &&
+                     (!res || (!p.out_fp32 && (reinterpret_cast<uintptr_t>(p.residual) & 15) == 0 && ldr % 16 == 0));
+    if (p.tma_epilogue) {
+        const uint64_t M = a->M, NE = (uint64_t)a->N * esz / 2, S = p.splits;
+        if (a->a_mode == 0) {
+            uint64_t dims[3] = {NE, M, S}, strides[2] = {ldd, M * ldd};
+            uint32_t box[3] = {32, BLOCK_M, 1};
+            CL_CHECK(get_tensor_map(&tD, dst, split ? 3 : 2, dims, strides, box, 64));
+            if (res) {
+                dims[0] = a->N;
+                CL_CHECK(get_tensor_map(&tR, p.residual, 2, dims, &ldr, box, 64));
+            }
+        } else {
+            const uint64_t Wo = p.Wo, Ho = p.Ho;
+            uint64_t dims[5] = {NE, Wo, Ho, (uint64_t)p.n_img, S};
+            uint32_t box[5] = {32, (uint32_t)p.bw, (uint32_t)p.bh, (uint32_t)p.bn, 1};
+            uint64_t strides[4] = {ldd, Wo * ldd, Ho * Wo * ldd, M * ldd};
+            CL_CHECK(get_tensor_map(&tD, dst, split ? 5 : 4, dims, strides, box, 64));
+            if (res) {
+                dims[0] = a->N;
+                uint64_t rs[3] = {ldr, Wo * ldr, Ho * Wo * ldr};
+                CL_CHECK(get_tensor_map(&tR, p.residual, 4, dims, rs, box, 64));
+            }
+        }
+    }
+
     const bool two = plan.occ == 2;
     int resident = 0;
     int* const q = info != nullptr ? &resident : nullptr;
-    const int st = dispatch_gemm(tA, tB, tE, p, stream, q, bn_sel, two, lora, BK);
+    const int st = dispatch_gemm(tA, tB, tE, tD, tR, p, stream, q, bn_sel, two, lora, BK);
     if (info != nullptr && st == CL_OK) { info[0] = bn_sel; info[1] = p.splits; info[2] = plan.occ; info[3] = resident; }
     return st;
 }
