@@ -548,11 +548,12 @@ splitk_finish_kernel(const float* __restrict__ ws, int splits, int M, int N, con
 // host side
 // =====================================================================================================
 
-// Launches the GEMM; with `resident` set, launches nothing and stores how many CTAs of this instantiation the device keeps
-// resident per SM at the shared-memory size the launch would use.
+// Launches the GEMM; with `plan` set, launches nothing and stores plan[0] = how many CTAs of this instantiation the device
+// keeps resident per SM at the shared-memory size the launch would use, plan[1] = the epilogue's store path (1: TMA,
+// 0: register stores).
 template <int BN, int EXT, int BK, int OCC>
 static int launch_gemm(const CUtensorMap& tA, const CUtensorMap& tB, const CUtensorMap& tE, const CUtensorMap& tD,
-                       const CUtensorMap& tR, const GemmParams& p_in, cudaStream_t stream, int* resident) {
+                       const CUtensorMap& tR, const GemmParams& p_in, cudaStream_t stream, int* plan) {
     using Cfg = GemmCfg<BN, EXT, BK>;
     constexpr int SMEM_LIMIT = GemmOcc<OCC>::SMEM_LIMIT;
     GemmParams p = p_in;
@@ -574,8 +575,9 @@ static int launch_gemm(const CUtensorMap& tA, const CUtensorMap& tB, const CUten
         CL_CUDA_CHECK(cudaFuncSetAttribute(gemm_wgmma_kernel<BN, EXT, BK, OCC>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
         attr_done = true;
     }
-    if (resident != nullptr) {
-        CL_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(resident, gemm_wgmma_kernel<BN, EXT, BK, OCC>, NUM_THREADS, smem_bytes));
+    if (plan != nullptr) {
+        CL_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&plan[0], gemm_wgmma_kernel<BN, EXT, BK, OCC>, NUM_THREADS, smem_bytes));
+        plan[1] = p.tma_epilogue ? 1 : 0;
         return CL_OK;
     }
     launch_k_pdl(gemm_wgmma_kernel<BN, EXT, BK, OCC>, (unsigned)grid, NUM_THREADS, smem_bytes, stream, tA, tB, tE, tD, tR, p,
@@ -694,7 +696,7 @@ static int dispatch_gemm(const CUtensorMap& tA, const CUtensorMap& tB, const CUt
     }
 }
 
-// cl_gemm, or with `info` set, cl_gemm_plan: info = {block_n, splits, ctas_per_sm, resident_per_sm} and no launch.
+// cl_gemm, or with `info` set, cl_gemm_plan: info = {block_n, splits, ctas_per_sm, resident_per_sm, tma_store} and no launch.
 static int run_gemm(const cl_gemm_args* a, cudaStream_t stream, int32_t* info) {
     if (a == nullptr || a->a == nullptr || a->b == nullptr || a->out == nullptr)
         return set_error(CL_ERR_INVALID, "cl_gemm: null pointer");
@@ -775,6 +777,14 @@ static int run_gemm(const cl_gemm_args* a, cudaStream_t stream, int32_t* info) {
         p.kb_per_split = (p.num_k_blocks + want - 1) / want;
         p.splits = (p.num_k_blocks + p.kb_per_split - 1) / p.kb_per_split;     // no empty split
         p.split_ws = reinterpret_cast<float*>(a->split_ws);
+        // the finishing kernel moves 4 columns per thread: 16-byte loads of the partials and the bias, 8 bytes of a bf16
+        // output or residual, 16 of an fp32 output
+        const uintptr_t ws = reinterpret_cast<uintptr_t>(a->split_ws), bi = reinterpret_cast<uintptr_t>(a->bias),
+                        rb = reinterpret_cast<uintptr_t>(a->row_bias), rs = reinterpret_cast<uintptr_t>(a->residual),
+                        out = reinterpret_cast<uintptr_t>(a->out);
+        if ((ws & 15) || (bi & 15) || (rb & 15) || (rs & 7) || (out & (a->out_fp32 ? 15 : 7)))
+            return set_error(CL_ERR_INVALID, "cl_gemm: split-K needs 16-byte aligned split_ws, bias, row_bias and fp32 out, "
+                                             "8-byte aligned bf16 out and residual");
     }
     {
         uint64_t dims[2] = {(uint64_t)a->K, (uint64_t)a->N};
@@ -838,10 +848,12 @@ static int run_gemm(const cl_gemm_args* a, cudaStream_t stream, int32_t* info) {
     }
 
     const bool two = plan.occ == 2;
-    int resident = 0;
-    int* const q = info != nullptr ? &resident : nullptr;
+    int launch_plan[2] = {0, 0};   // resident CTAs per SM, store path
+    int* const q = info != nullptr ? launch_plan : nullptr;
     const int st = dispatch_gemm(tA, tB, tE, tD, tR, p, stream, q, bn_sel, two, lora, BK);
-    if (info != nullptr && st == CL_OK) { info[0] = bn_sel; info[1] = p.splits; info[2] = plan.occ; info[3] = resident; }
+    if (info != nullptr && st == CL_OK) {
+        info[0] = bn_sel; info[1] = p.splits; info[2] = plan.occ; info[3] = launch_plan[0]; info[4] = launch_plan[1];
+    }
     return st;
 }
 

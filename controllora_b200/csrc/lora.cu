@@ -146,9 +146,12 @@ skinny_atb_batch_kernel(const __grid_constant__ SkinnyBatch batch, int slabs) {
                 const long long mc = ok ? mk : (row1 - 1);      // clamp: a padded row contributes with zero coefficients
                 u[k] = __ldg(reinterpret_cast<const uint4*>(b + mc * d.ldb));
                 if (vec_a) {
+                    // only the 4-column groups that hold one of the r columns: at RT = 8, a rank-4 t[:, 4:] view of an
+                    // [M, 8] table would otherwise read 16 bytes past the table's last row
 #pragma unroll
                     for (int q = 0; q < RT / 4; ++q) {
-                        const float4 t4 = __ldg(reinterpret_cast<const float4*>(a + mc * d.lda + 4 * q));
+                        const float4 t4 = 4 * q < R ? __ldg(reinterpret_cast<const float4*>(a + mc * d.lda + 4 * q))
+                                                    : make_float4(0.f, 0.f, 0.f, 0.f);
                         av[k][4 * q] = ok ? t4.x : 0.f; av[k][4 * q + 1] = ok ? t4.y : 0.f;
                         av[k][4 * q + 2] = ok ? t4.z : 0.f; av[k][4 * q + 3] = ok ? t4.w : 0.f;
                     }

@@ -6,7 +6,10 @@ Every reference is computed in fp64 on the device from the same bf16-rounded inp
 written as a view inside a larger buffer filled with a sentinel bit pattern, with sentinel columns beside the view and
 sentinel rows after its last row: after the kernel, every sentinel must be bit-identical (a store masked one element too
 wide, or landing in the wrong row, column or third of a fused buffer, shows up there and nowhere else).  Each GEMM case records the plan the launcher took (cl_gemm_plan) and asserts the one
-it was written for, so a planner change fails here instead of moving the case to another kernel.
+it was written for, so a planner change fails here instead of moving the case to another kernel.  It also asserts the
+epilogue's store path (cl_gemm_plan's fifth entry: TMA stores from shared memory, or register stores for outputs and
+residuals that are not 16-byte aligned and fp32 outputs with a residual): every instantiation runs on both, and the two
+must agree bit for bit.
 
 Error bounds, per element, from the arithmetic the kernels perform (T = the fp64 sum of |terms| of the element):
   - fp32 accumulation of exact bf16 products (wgmma, fp32 FMA chains): every addition loses at most one fp32 ulp of the
@@ -35,7 +38,7 @@ Error bounds, per element, from the arithmetic the kernels perform (T = the fp64
     gradient; each test states its terms.  dgamma / dbeta are fp32 reductions (assert_f32_reduction).
 
 `test_every_gemm_instantiation_has_a_case` and `test_every_head_dim_has_a_case` (no GPU needed) parse the dispatch
-tables and fail when an instantiation has no case here.
+tables and fail when an instantiation, or an (instantiation, store path) pair, has no case here.
 """
 from __future__ import annotations
 
@@ -189,8 +192,10 @@ def _conv_n(S, per_image):
     return math.ceil(2 * S / per_image)
 
 
-# A case: dict(M, N, K) for a matrix A or conv=(n, H, W, C, stride, pad_lo) with N; the epilogue inputs; want = the plan
-# (BK, BN, lora, split, ctas_per_sm) where split is 1, ">1" (any split) or an exact count.  Builders take the SM count.
+# A case: dict(M, N, K) for a matrix A or conv=(n, H, W, C, stride, pad_lo) with N; the epilogue inputs; store = the
+# epilogue's store path ("tma" unless given: the output canvas is 16-byte aligned with a 16-byte multiple pitch when N % 8
+# == 0); want = the plan (BK, BN, lora, split, ctas_per_sm) where split is 1, ">1" (any split) or an exact count.
+# Builders take the SM count.
 def _g(name, want, **kw):
     return pytest.param(kw, want, id=name)
 
@@ -224,12 +229,12 @@ GEMM_TAIL_CASES = [
     _g("m_tail_1", (64, 64, False, 1, 1), M=1025, N=320, K=320, bias=True, residual="alias"),
     _g("m_tail_64", (64, 64, False, 1, 1), M=1088, N=320, K=320, row_bias=100, out_fp32=True),
     _g("m_tail_127", (64, 64, False, 1, 1), M=1151, N=320, K=320, bias=True, row_bias=77, residual="sep"),
-    _g("n_tail_100_k200", (64, 128, False, 1, 1), M=1001, N=100, K=200, bias=True, residual="sep"),
+    _g("n_tail_100_k200", (64, 128, False, 1, 1), M=1001, N=100, K=200, bias=True, residual="sep", store="reg"),
     _g("n_tail_200_k72", (64, 160, False, 1, 1), M=1153, N=200, K=72, bias=True, row_bias=300),
     _g("n_tail_1000_k8", (64, 160, False, 1, 1), M=129, N=1000, K=8, out_fp32=True, bias=True),
-    _g("n_tail_36", (64, 64, False, 1, 1), M=1000, N=36, K=64, residual="alias"),
+    _g("n_tail_36", (64, 64, False, 1, 1), M=1000, N=36, K=64, residual="alias", store="reg"),
     _g("lora_r8_tails", (64, 160, True, 1, 1), M=1025, N=200, K=72, lora=8, t_add=True, t_out=True, bias=True),
-    _g("lora_r4_tails", (64, 160, True, 1, 1), M=1151, N=100, K=200, lora=4, t_out=True, residual="alias"),
+    _g("lora_r4_tails", (64, 160, True, 1, 1), M=1151, N=100, K=200, lora=4, t_out=True, residual="alias", store="reg"),
     _g("lora_r4_text", (64, 64, True, 1, 1), M=154, N=768, K=768, lora=4, t_add=True, t_out=True),
     # conv pixel tiles: Wo = 1, 2, 4, 12, 24, 48, 96 (bw x bh x bn = 1x1x128, 2x2x32, 4x4x8, 4x4x8, 8x8x2, 16x8x1, 32x4x1)
     _g("conv_wo1", (64, 64, False, 1, 1), conv=lambda S: (3, 1, 1, 64, 1, 1), N=64, bias=True, residual="sep"),
@@ -261,7 +266,7 @@ GEMM_SPLIT_CASES = [
     _g("conv_s2_split4", (64, 64, False, 4, 1), conv=lambda S: (2, 16, 16, 256, 2, 0), N=256, bias=True, out_fp32=True),
 ]
 
-REACHED = {"gemm": set(), "d16": set(), "gn": set()}
+REACHED = {"gemm": set(), "gemm_store": set(), "d16": set(), "gn": set()}
 
 
 def _plan_splits(rows):
@@ -309,11 +314,15 @@ def _recording(cap=0):
         _lib._lib, ops._split_ws = real, real_ws
 
 
-def _run_gemm_case(spec, want):
+def _run_gemm_case(spec, want, register_store=False):
+    """Runs one case and checks it against fp64; returns the output.  register_store: the output view starts 8 bytes
+    into a 16-byte unit (column 4 of a bf16 canvas, 2 of an fp32 one), so the epilogue must take the register stores; the
+    inputs are those of the aligned run (the seed does not depend on the store)."""
     from controllora_b200 import ops
 
     S = _sms()
     spec = {k: (v(S) if callable(v) else v) for k, v in spec.items()}
+    store = spec.pop("store", "tma")
     _seed("gemm", sorted((k, str(v)) for k, v in spec.items()))
     N = spec["N"]
     conv = spec.get("conv")
@@ -331,7 +340,10 @@ def _run_gemm_case(spec, want):
     b = _bf(N, K, scale=K**-0.5)
     out_fp32 = bool(spec.get("out_fp32"))
     odt = F32 if out_fp32 else BF16
-    cout = Canvas((M + 3, N + 24), odt, (slice(1, 1 + M), slice(8, 8 + N)))      # ldd > N, column offset 8
+    c0 = (4 if odt == BF16 else 2) if register_store else 8
+    if register_store:
+        store = "reg"
+    cout = Canvas((M + 3, N + 24), odt, (slice(1, 1 + M), slice(c0, c0 + N)))    # ldd > N, column offset 8 (or 8 bytes)
     out = cout.view
     out0 = None
     bias = _f32(N) if spec.get("bias") else None
@@ -388,7 +400,10 @@ def _run_gemm_case(spec, want):
     wsplit = want[3]
     ok = got[:3] == want[:3] and got[4] == want[4] and (got[3] == wsplit if isinstance(wsplit, int) else got[3] > 1)
     assert ok, f"planned {got}, the case was written for {want}"
+    tma = {"tma": 1, "reg": 0}[store]
+    assert plan[4] == tma, f"plan {got} takes the {('register', 'TMA')[plan[4]]} store, the case was written for {store}"
     REACHED["gemm"].add((BK, plan[0], bool(lora), plan[1] > 1, plan[2]))
+    REACHED["gemm_store"].add((_inst_of(got), store))
     if len(outs) > 1:
         assert torch.equal(outs[0].view(torch.int16 if odt == BF16 else torch.int32),
                            outs[1].view(torch.int16 if odt == BF16 else torch.int32)), "two runs differ"
@@ -436,12 +451,13 @@ def _run_gemm_case(spec, want):
         acc = acc + r0
         T = T + r0.abs()
     E = E + ACC * (K + 4) * T
-    what = f"gemm plan {got}"
+    what = f"gemm plan {got}, {store} store"
     if out_fp32:
         assert_f32_within(out, acc, E, what + " (fp32 out) vs fp64")
     else:
         assert_bf16_within(out, acc, E, what + " vs fp64")
     cout.check(what)
+    return out.clone(), store
 
 
 @gpu
@@ -475,6 +491,120 @@ def test_every_gemm_instantiation_has_a_case():
     assert not missing, f"launch_gemm instantiations without a case in {Path(__file__).name}: {missing}"
     extra = sorted(cased - set(table))
     assert not extra, f"cases for instantiations dispatch_gemm no longer has: {extra}"
+    pairs = {(_inst_of(p.values[1]), p.values[0].get("store", "tma"))
+             for p in GEMM_INSTANTIATION_CASES + GEMM_TAIL_CASES + GEMM_SPLIT_CASES + GEMM_FP32_RESIDUAL_CASES}
+    pairs |= {(_inst_of(p.values[1]), "reg") for p in GEMM_REGISTER_STORE_CASES}
+    missing = sorted({(i, st) for i in table for st in ("tma", "reg")} - pairs)
+    assert not missing, f"(launch_gemm instantiation, store path) pairs without a case in {Path(__file__).name}: {missing}"
+    assert all(p.values[1][3] == 1 for p in GEMM_REGISTER_STORE_CASES), "split-K partials always leave by TMA"
+
+
+# ---- the register-store epilogue.  Every instantiation's case again, and convs with tails, LoRA tails and an M tail,
+# with the output view 8 bytes off a 16-byte unit: the launch must take the register stores and give the TMA run's bits
+# (both add bias, row bias and residual in the same fp32 order).  fp32 outputs with a residual always take them.
+GEMM_REGISTER_STORE_CASES = GEMM_INSTANTIATION_CASES + [
+    p for p in GEMM_TAIL_CASES if p.id in ("m_tail_127", "lora_r8_tails", "lora_r4_text", "conv_wo1", "conv_wo4_c96",
+                                            "conv_s2_wo12_c96_pad1", "conv_s2_wo1_pad1")]
+GEMM_FP32_RESIDUAL_CASES = [
+    _g("fp32_residual_bn64", (64, 64, False, 1, 1), M=1000, N=320, K=320, out_fp32=True, bias=True, row_bias=300,
+       residual="sep", store="reg"),
+    _g("fp32_residual_bn160_occ2", (64, 160, False, 1, 2), M=lambda S: _m2(S, 2), N=320, K=320, out_fp32=True, bias=True,
+       row_bias=2000, residual="sep", store="reg"),
+    _g("fp32_residual_conv_bk32", (32, 32, False, 1, 1), conv=lambda S: (3, 24, 24, 32, 1, 1), N=64, out_fp32=True,
+       bias=True, row_bias=576, residual="sep", store="reg"),
+    _g("fp32_residual_lora", (64, 64, True, 1, 1), M=1024, N=640, K=640, lora=4, t_out=True, out_fp32=True, bias=True,
+       residual="sep", store="reg"),
+]
+
+
+@gpu
+@pytest.mark.parametrize("spec,want", GEMM_REGISTER_STORE_CASES)
+def test_gemm_register_store(spec, want):
+    out_a, store_a = _run_gemm_case(spec, want)
+    out_r, store_r = _run_gemm_case(spec, want, register_store=True)
+    assert store_r == "reg"
+    it = torch.int16 if out_a.dtype == BF16 else torch.int32
+    assert torch.equal(out_a.view(it), out_r.view(it)), f"the {store_a} and register stores give different bits"
+
+
+@gpu
+@pytest.mark.parametrize("spec,want", GEMM_FP32_RESIDUAL_CASES)
+def test_gemm_fp32_output_with_residual(spec, want):
+    _run_gemm_case(spec, want)
+
+
+class _PlanOnly:
+    """Stands in for the ctypes library: cl_gemm returns cl_gemm_plan's status and records its plan; nothing launches."""
+
+    def __init__(self, real):
+        self.real, self.plans = real, []
+
+    def __getattr__(self, name):
+        return getattr(self.real, name)
+
+    def cl_gemm(self, pargs, stream):
+        info = (ct.c_int32 * 5)()
+        st = self.real.cl_gemm_plan(pargs, info)
+        self.plans.append((st, tuple(info)))
+        return st
+
+
+def _plan_only(spec, out_fp32, split_ws=None):
+    """(status, cl_gemm_plan info) of a case's shape with uninitialised operands and an aligned output."""
+    from controllora_b200 import _lib, ops
+
+    S = _sms()
+    spec = {k: (v(S) if callable(v) else v) for k, v in spec.items()}
+    N = spec["N"]
+    kw = {}
+    if spec.get("conv"):
+        n, H, W, Cc, stride, pad_lo = spec["conv"]
+        K = 9 * Cc
+        a = torch.empty(n, H, W, Cc, device="cuda", dtype=BF16)
+        kw.update(conv_stride=stride, pad_lo=pad_lo)
+    else:
+        K = spec["K"]
+        a = torch.empty(spec["M"], K, device="cuda", dtype=BF16)
+    if spec.get("lora"):
+        kw.update(ext=torch.zeros(16, K, device="cuda", dtype=BF16), lora_up=torch.zeros(N, spec["lora"], device="cuda"))
+    real, real_ws = _lib.lib(), ops._split_ws
+    rec = _PlanOnly(real)
+    _lib._lib = rec
+    if split_ws is not None:
+        ops._split_ws = split_ws
+    try:
+        ops.gemm(a, torch.empty(N, K, device="cuda", dtype=BF16), out_fp32=out_fp32, **kw)
+        ((st, info),) = rec.plans
+    finally:
+        _lib._lib, ops._split_ws = real, real_ws
+    return st, info
+
+
+@gpu
+@pytest.mark.parametrize("out_fp32", [False, True])
+def test_gemm_staged_tile_fits_every_ring(out_fp32):
+    """launch_gemm falls back to the register stores when the staged output tile (fp32 for split-K partials and fp32
+    outputs) does not fit the ring.  At every instantiation's stage count it fits, so an aligned output must take TMA;
+    a stage or tile change that makes the fallback reachable fails here and needs register-store cases of its own."""
+    for p in GEMM_INSTANTIATION_CASES + GEMM_SPLIT_CASES:
+        spec, want = p.values
+        st, info = _plan_only(spec, out_fp32)
+        assert st == 0, f"{p.id}: cl_gemm_plan status {st}"
+        assert (info[0], info[2]) == (want[1], want[4]), f"{p.id}: plan {tuple(info)}"
+        assert info[4] == 1, f"{p.id} (out_fp32 {out_fp32}): the staged tile does not fit the ring, plan {tuple(info)}"
+
+
+@gpu
+def test_gemm_split_k_rejects_a_misaligned_workspace():
+    """The split-K finishing kernel reads the partials 16 bytes at a time: a workspace 8 bytes off is an argument
+    error (checked through the plan, nothing launches)."""
+    from controllora_b200 import _lib
+
+    spec, want = next(p.values for p in GEMM_SPLIT_CASES if p.id == "split16")
+    st, info = _plan_only(spec, False)
+    assert st == 0 and info[1] == 16 and info[4] == 1, info
+    with pytest.raises(_lib.CLError, match="split-K needs 16-byte aligned"):
+        _plan_only(spec, False, split_ws=lambda numel, device: torch.empty(numel + 4, device=device)[2:2 + numel])
 
 
 # ====================================================================================================== attention

@@ -26,10 +26,10 @@ SHORT_K = 20   # k-blocks per tile at or below which a launch counts as short-K
 
 
 def _plan(lib, args):
-    """(block_n, splits, ctas_per_sm, resident_per_sm), or None for a library without cl_gemm_plan."""
+    """(block_n, splits, ctas_per_sm, resident_per_sm, tma_store), or None for a library without cl_gemm_plan."""
     if not hasattr(lib, "cl_gemm_plan"):
         return None
-    info = (C.c_int32 * 4)()
+    info = (C.c_int32 * 5)()
     if lib.cl_gemm_plan(C.byref(args), info) != 0:
         return None
     return tuple(info)
@@ -242,7 +242,7 @@ def main():
     print(f"{'M':>7} {'N':>6} {'K':>6} {'mode':>4} {'lora':>4} {'kb/tile':>7} {'bn':>4} {'spl':>3} {'cta/SM':>6} {'resident':>8} "
           f"{'count':>5} {'step us':>9} {'alone us':>9}")
     for d in sorted(distinct.values(), key=lambda d: -d["step_us"]):
-        k, p = d["key"], d["plan"] or (0, 0, 0, 0)
+        k, p = d["key"], d["plan"] or (0, 0, 0, 0, 0)
         print(f"{k['M']:7d} {k['N']:6d} {k['K']:6d} {k['a_mode']:4d} {k['lora_rp']:4d} {d['kb_per_tile']:7d} {p[0]:4d} {p[1]:3d} "
               f"{p[2]:6d} {p[3]:8d} {d['count']:5d} {d['step_us']:9.1f} {d['alone_us']:9.1f}")
     print(f"GEMM launches in one step: {len(rows)}, {total / 1e3:.3f} ms (serialised event timing); "
