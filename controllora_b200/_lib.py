@@ -48,6 +48,8 @@ def lib() -> C.CDLL:
         _lib.cl_cfg_plms_step_dev.restype = C.c_int
         _lib.cl_cfg_plms_step_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                               C.c_float, C.c_void_p]
+        _lib.cl_cfg_plms_step_v_dev.restype = C.c_int
+        _lib.cl_cfg_plms_step_v_dev.argtypes = list(_lib.cl_cfg_plms_step_dev.argtypes)
     return _lib
 
 

@@ -5,10 +5,11 @@
 
 Forward only (the reference freezes it, train_…:431).  SD-1.5 `text_encoder/config.json` = CLIP ViT-L/14 text tower: 12 pre-LN
 transformer layers of width 768, 12 heads of 64, MLP 3072 with `quick_gelu`, 77 learned positions, vocabulary 49408, causal
-self-attention, final LayerNorm; `[0]` of the output = `last_hidden_state` [B, 77, 768].  Per layer: LayerNorm kernel -> ONE
+self-attention, final LayerNorm; `[0]` of the output = `last_hidden_state` [B, 77, 768].  SD-2.x (SD21_TEXT_CONFIG): 23 layers of
+width 1024, 16 heads of 64, MLP 4096 with the exact erf `gelu` (cl_gelu), output [B, 77, 1024].  Per layer: LayerNorm kernel -> ONE
 fused q|k|v projection (N = 2304, bias in the GEMM epilogue) -> causal attention of the 77-token sequence (one CTA per
 (batch, head), fp32 online softmax) -> out-projection with bias + residual in the epilogue -> LayerNorm -> fc1 (+bias) ->
-quick_gelu -> fc2 (+bias, +residual).  State-dict keys = transformers' `CLIPTextModel` (`text_model.embeddings.…`,
+quick_gelu or gelu -> fc2 (+bias, +residual).  State-dict keys = transformers' `CLIPTextModel` (`text_model.embeddings.…`,
 `text_model.encoder.layers.{i}.…`, `text_model.final_layer_norm.…`).  Tokenisation stays with `transformers.CLIPTokenizer`
 (host-side string processing, not part of this path).
 """
@@ -27,6 +28,12 @@ BF16 = torch.bfloat16
 
 SD15_TEXT_CONFIG = dict(vocab_size=49408, hidden_size=768, intermediate_size=3072, num_hidden_layers=12, num_attention_heads=12,
                         max_position_embeddings=77, layer_norm_eps=1e-5, hidden_act="quick_gelu")
+# SD-2.x text encoder (OpenCLIP ViT-H/14's text tower in transformers format, `text_encoder/config.json` of SD-2-base and SD-2.1):
+# width 1024, 16 heads of 64, MLP 4096 with the exact erf `gelu`, 23 layers (the diffusers conversion drops the last of
+# OpenCLIP's 24, so `[0]` = last_hidden_state is the penultimate-layer output the SD-2 pipelines condition on).
+SD21_TEXT_CONFIG = dict(SD15_TEXT_CONFIG, hidden_size=1024, intermediate_size=4096, num_hidden_layers=23, num_attention_heads=16,
+                        hidden_act="gelu")
+_ACTIVATIONS = {"quick_gelu": "quick_gelu_", "gelu": "gelu_"}
 
 
 class _Layer:
@@ -49,8 +56,10 @@ class CLIPTextModel(nn.Module):
         super().__init__()
         cfg = dict(SD15_TEXT_CONFIG)
         cfg.update(config or {})
-        if cfg["hidden_act"] != "quick_gelu":
-            raise NotImplementedError("CLIPTextModel: only the quick_gelu MLP of SD-1.5's text encoder is implemented")
+        if cfg["hidden_act"] not in _ACTIVATIONS:
+            raise NotImplementedError(f"CLIPTextModel: hidden_act {cfg['hidden_act']!r} is not implemented (quick_gelu: SD-1.5, "
+                                      f"gelu: SD-2.x)")
+        self._act = _ACTIVATIONS[cfg["hidden_act"]]
         self.config = SimpleNamespace(**cfg)
         dev = torch.device(device)
         from ._lib import require_cuda
@@ -145,7 +154,7 @@ class CLIPTextModel(nn.Module):
             a = ops.causal_attention_small(qkv, B, T, self.heads, scale)
             x = ops.gemm(a, L.w_o, bias=L.b_o, residual=x)
             h, _ = ops.layernorm_fwd(x, L.ln2[0], L.ln2[1], cfg.layer_norm_eps)
-            f = ops.quick_gelu_(ops.gemm(h, L.w_fc1, bias=L.b_fc1))
+            f = getattr(ops, self._act)(ops.gemm(h, L.w_fc1, bias=L.b_fc1))
             x = ops.gemm(f, L.w_fc2, bias=L.b_fc2, residual=x)
         y, _ = ops.layernorm_fwd(x, self.ln_f[0], self.ln_f[1], cfg.layer_norm_eps)
         y = y.view(B, T, Cw)

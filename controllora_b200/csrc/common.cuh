@@ -198,6 +198,25 @@ __device__ __forceinline__ float2 unpack_bf16x2(uint32_t u) {
     return __bfloat1622float2(t);
 }
 
+// Step counter of the graph-replayable sampler steps that advance it in the same launch: every CTA reads the step from the
+// low 32 bits of *step_ctr (sampler_step_read), and after __syncthreads (every thread of the CTA has read it) counts itself in
+// the high 32 bits; the last CTA to arrive clears them and adds 1 to the step (sampler_step_arrive).  No CTA can observe the
+// new step, because it is written only after every CTA has read the old one.
+__device__ __forceinline__ unsigned long long sampler_step_read(unsigned long long* step_ctr) {
+    return *reinterpret_cast<volatile unsigned long long*>(step_ctr) & 0xffffffffull;
+}
+__device__ __forceinline__ void sampler_step_arrive(unsigned long long* step_ctr) {
+    if (threadIdx.x == 0) {
+        constexpr unsigned long long ARRIVE = 1ull << 32;
+        const unsigned long long old = atomicAdd(step_ctr, ARRIVE);
+        if ((old >> 32) == (unsigned long long)gridDim.x - 1ull)
+            atomicAdd(step_ctr, 1ull - (unsigned long long)gridDim.x * ARRIVE);   // arrivals -> 0, step + 1 (mod 2^64)
+    }
+}
+
+// exact erf GELU (GEGLU's gate in the UNet, the MLP activation of SD-2's text tower)
+__device__ __forceinline__ float gelu_f(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
+
 // (a, b) -> bf16x2 of the rounded values and bf16x2 of the rounding residuals: a ~= hi.x + lo.x to ~2^-17 relative
 __device__ __forceinline__ void split_bf16x2(float a, float b, uint32_t& hi, uint32_t& lo) {
     hi = pack_bf16x2(a, b);

@@ -33,7 +33,6 @@ static inline int ew_blocks(long long work, int threads = 256) {
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < (n); i += (long long)gridDim.x * blockDim.x)
 
 // ---------------------------------------------------------------- GEGLU: out = a * gelu_erf(g), p = [a | g]
-__device__ __forceinline__ float gelu_f(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
 __device__ __forceinline__ float gelu_grad_f(float x) {
     return 0.5f * (1.f + erff(x * 0.70710678118654752f)) + x * 0.3989422804014327f * __expf(-0.5f * x * x);
 }

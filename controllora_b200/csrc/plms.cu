@@ -13,9 +13,7 @@
 //               x <- sample_coeff s + eps_coeff e';  (r3, r2, r1) <- (r2, r1, e) if push.
 // Each thread owns its elements of x, the ring and the saved sample, so the in-place updates need no synchronisation.
 //
-// The step counter advances in the same launch: every CTA reads the step from the low 32 bits of *step_ctr, then counts
-// itself in the high 32 bits; the last CTA to arrive clears them and adds 1 to the step.  No CTA can observe the new
-// step, because it is written only after every CTA has read the old one.
+// The step counter advances in the same launch (sampler_step_read / sampler_step_arrive in common.cuh).
 #include "common.cuh"
 #include "host_common.h"
 #include "../../include/controllora_b200.h"
@@ -28,8 +26,7 @@ cfg_plms_dev_kernel(const float* __restrict__ eps2, float* __restrict__ x, float
                     long long n_half, float g) {
     pdl_launch_dependents();
     pdl_wait();
-    const unsigned long long step = *reinterpret_cast<volatile unsigned long long*>(step_ctr) & 0xffffffffull;
-    const float* row = rows + 8 * step;
+    const float* row = rows + 8 * sampler_step_read(step_ctr);
     const float sc = row[1], ec = row[2], w0 = row[3], w1 = row[4], w2 = row[5], w3 = row[6];
     const int flags = (int)row[7];
     const bool push = flags & 1, save = flags & 2, restart = flags & 4;
@@ -51,12 +48,7 @@ cfg_plms_dev_kernel(const float* __restrict__ eps2, float* __restrict__ x, float
         }
     }
     __syncthreads();                                  // every thread of this CTA has read the step
-    if (threadIdx.x == 0) {
-        constexpr unsigned long long ARRIVE = 1ull << 32;
-        const unsigned long long old = atomicAdd(step_ctr, ARRIVE);
-        if ((old >> 32) == (unsigned long long)gridDim.x - 1ull)
-            atomicAdd(step_ctr, 1ull - (unsigned long long)gridDim.x * ARRIVE);   // arrivals -> 0, step + 1 (mod 2^64)
-    }
+    sampler_step_arrive(step_ctr);
 }
 
 }  // namespace clb

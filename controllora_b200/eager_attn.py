@@ -35,13 +35,13 @@ class _Binding:
     def __init__(self, proc, attn):
         w = attn.to_q.weight
         require_cuda(w.device, "processor call")
-        # the SD-1.5 flavour of diffusers' CrossAttention only (what the reference runs on): no group norm, no added k/v projections,
-        # no up-cast attention, biased output projection
+        # the SD-1.5 / SD-2.x flavour of diffusers' CrossAttention only (what the reference runs on): no group norm, no added k/v
+        # projections, biased output projection.  upcast_attention / upcast_softmax (set by some SD-2.x UNets) ask for QK^T and
+        # the softmax in fp32; the attention kernels always compute QK^T from the bf16 operands with fp32 accumulation and the
+        # softmax in fp32, so up-cast modules run unchanged.
         for attr, what in (("group_norm", "group-normalised"), ("added_kv_proj_dim", "added-kv")):
             if getattr(attn, attr, None) is not None:
                 raise NotImplementedError(f"controllora_b200 processors: {what} attention modules are outside the SD-1.5 path")
-        if getattr(attn, "upcast_attention", False) or getattr(attn, "upcast_softmax", False):
-            raise NotImplementedError("controllora_b200 processors: up-cast attention is outside the SD-1.5 path")
         if attn.to_q.bias is not None or attn.to_out[0].bias is None:
             raise NotImplementedError("controllora_b200 processors: expected to_q/to_k/to_v without bias and a biased to_out[0]")
         sd = {"to_q.weight": attn.to_q.weight.detach(), "to_k.weight": attn.to_k.weight.detach(),

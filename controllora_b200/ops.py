@@ -675,6 +675,14 @@ def quick_gelu_(x):
     return x
 
 
+def gelu_(x):
+    """in place: the exact erf GELU 0.5 x (1 + erf(x / sqrt 2)) (bf16, numel % 8 == 0)."""
+    _req(x, BF16, "x")
+    assert x.is_contiguous()
+    _call("cl_gelu", _p(x), C.c_int64(x.numel()))
+    return x
+
+
 def causal_attention_small(qkv, B: int, T: int, heads: int, scale: float):
     """causal softmax(q k^T * scale) v of a short sequence; qkv [B*T, 3*C] bf16 (q | k | v) -> [B*T, C] bf16."""
     _req(qkv, BF16, "qkv")
@@ -740,6 +748,28 @@ def cfg_plms_step_dev(eps2, latents, ring, saved, rows, step_ctr, guidance: floa
     assert eps2.numel() == 2 * n and ring.numel() == 3 * n and saved.numel() == n
     assert rows.dim() == 2 and rows.shape[1] == 8 and step_ctr.dtype == torch.int64 and step_ctr.numel() == 1
     _call("cl_cfg_plms_step_dev", _p(eps2), _p(latents), _p(ring), _p(saved), _p(rows), _p(step_ctr), n, float(guidance))
+
+
+def cfg_solver_step_v_dev(v2, latents, x0_prev, coef, step_ctr, guidance: float, kind: int):
+    """cfg_solver_step_dev for a v-prediction model: v2 [2B, ...] fp32 = [uncond | cond] model outputs, the same coef rows."""
+    _req(v2, torch.float32, "v2")
+    _req(latents, torch.float32, "latents")
+    assert v2.is_contiguous() and latents.is_contiguous() and v2.numel() == 2 * latents.numel()
+    assert coef.dtype == torch.float32 and coef.is_contiguous() and coef.shape[1] == 8 and step_ctr.dtype == torch.int64
+    _call("cl_cfg_solver_step_v_dev", _p(v2), _p(latents), _p(x0_prev), _p(coef), _p(step_ctr), C.c_int64(latents.numel()),
+          C.c_float(guidance), int(kind))
+
+
+def cfg_plms_step_v_dev(v2, latents, ring, saved, rows, step_ctr, guidance: float):
+    """cfg_plms_step_dev for a v-prediction model: the ring holds guided v outputs, rows are the 10-column
+    sampler.pndm_rows(..., prediction_type="v_prediction")."""
+    for t, name in ((v2, "v2"), (latents, "latents"), (ring, "ring"), (saved, "saved"), (rows, "rows")):
+        _req(t, torch.float32, name)
+        assert t.is_contiguous(), name
+    n = latents.numel()
+    assert v2.numel() == 2 * n and ring.numel() == 3 * n and saved.numel() == n
+    assert rows.dim() == 2 and rows.shape[1] == 10 and step_ctr.dtype == torch.int64 and step_ctr.numel() == 1
+    _call("cl_cfg_plms_step_v_dev", _p(v2), _p(latents), _p(ring), _p(saved), _p(rows), _p(step_ctr), n, float(guidance))
 
 
 class SkinnyQueue:

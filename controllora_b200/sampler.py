@@ -44,6 +44,28 @@ def _check_control(control_lora, guide) -> None:
         raise ValueError("pass control_lora and guide together, or neither of them (sampling without a ControlLoRA)")
 
 
+PREDICTION_TYPES = ("epsilon", "v_prediction")
+
+
+def _check_prediction_type(prediction_type: str) -> None:
+    if prediction_type not in PREDICTION_TYPES:
+        raise ValueError(f"unknown prediction_type {prediction_type!r}: expected one of {PREDICTION_TYPES}")
+
+
+def scheduler_prediction_type(pretrained_model_name_or_path, subfolder: str = "scheduler") -> str:
+    """`prediction_type` of a local diffusers checkpoint's `<root>/<subfolder>/scheduler_config.json` ("epsilon" when the key is
+    absent, diffusers' default) - what train_text_to_image_control_lora.py:774-779 reads from `noise_scheduler.config`.  SD-1.5 and
+    SD-2-base give "epsilon", SD-2.1 (768) gives "v_prediction".  Nothing else of the file is read."""
+    import json
+    import os
+
+    path = os.path.join(str(pretrained_model_name_or_path), subfolder, "scheduler_config.json")
+    with open(path) as f:
+        value = json.load(f).get("prediction_type", "epsilon")
+    _check_prediction_type(value)
+    return value
+
+
 def _begin_loop(control_lora, guide, cond, uncond, latents, seed, height, width):
     """Start of every eager loop: initial latents (seeded CPU draw unless given), `control_lora(guide)` tiled to the CFG batch
     when there is a ControlLoRA, and the [uncond | cond] text states.  Without a ControlLoRA (control_lora = guide = None) the
@@ -70,10 +92,14 @@ def _begin_loop(control_lora, guide, cond, uncond, latents, seed, height, width)
 @torch.no_grad()
 def ddim_sample(unet, control_lora, guide: Optional[torch.Tensor], cond: torch.Tensor, uncond: torch.Tensor, num_inference_steps: int = 50,
                 guidance_scale: float = 7.5, latents: Optional[torch.Tensor] = None, seed: int = 0, height: int = 512,
-                width: int = 512) -> torch.Tensor:
+                width: int = 512, prediction_type: str = "epsilon") -> torch.Tensor:
     """guide [B,3,H,W] in [-1,1]; cond / uncond text states [B,77,D] bf16.  Returns the final latents [B,4,H/8,W/8] fp32.
-    control_lora = guide = None samples without a ControlLoRA (height / width then give the image size unless latents do)."""
+    control_lora = guide = None samples without a ControlLoRA (height / width then give the image size unless latents do).
+    prediction_type "v_prediction" reads the UNet output as v (SD-2.1 768), with the step scalars from a device table."""
+    _check_prediction_type(prediction_type)
     B, dev, latents, ehs = _begin_loop(control_lora, guide, cond, uncond, latents, seed, height, width)
+    if prediction_type == "v_prediction":
+        return _v_solver_loop(unet, 0, num_inference_steps, guidance_scale, latents, ehs)
     ac = sd15_alphas_cumprod()
     for t in ddim_timesteps(num_inference_steps):
         x2 = torch.cat([latents, latents], 0)
@@ -122,9 +148,12 @@ def dpmpp_2m_coeffs(i: int, timesteps: List[int], ac: List[float], lower_order_f
 @torch.no_grad()
 def dpmpp_sample(unet, control_lora, guide: Optional[torch.Tensor], cond: torch.Tensor, uncond: torch.Tensor, num_inference_steps: int = 30,
                  guidance_scale: float = 7.5, latents: Optional[torch.Tensor] = None, seed: int = 0, height: int = 512,
-                 width: int = 512) -> torch.Tensor:
+                 width: int = 512, prediction_type: str = "epsilon") -> torch.Tensor:
     """Same contract as ddim_sample with the DPM-Solver++(2M) update; one fused CFG + solver kernel per step."""
+    _check_prediction_type(prediction_type)
     B, dev, latents, ehs = _begin_loop(control_lora, guide, cond, uncond, latents, seed, height, width)
+    if prediction_type == "v_prediction":
+        return _v_solver_loop(unet, 1, num_inference_steps, guidance_scale, latents, ehs)
     x0_prev = torch.zeros_like(latents)
     ac = sd15_alphas_cumprod()
     ts = dpm_timesteps(num_inference_steps)
@@ -134,6 +163,38 @@ def dpmpp_sample(unet, control_lora, guide: Optional[torch.Tensor], cond: torch.
         eps2 = unet(x2, tt, ehs).sample
         a_s, sg_s, c_x, c_m0, c_m1 = dpmpp_2m_coeffs(i, ts, ac)
         ops.cfg_dpmpp_step(eps2, latents, x0_prev, guidance_scale, a_s, sg_s, c_x, c_m0, c_m1)
+    return latents
+
+
+def solver_table(kind: int, num_inference_steps: int) -> Tuple[List[int], List[List[float]]]:
+    """(UNet timesteps, coef rows [steps][8]) of the device-table step: kind 0 = DDIM (sqrt_at, sqrt_1m_at, sqrt_aprev,
+    sqrt_1m_aprev), kind 1 = DPM-Solver++(2M) (dpmpp_2m_coeffs).  The rows serve both prediction types."""
+    ac = sd15_alphas_cumprod()
+    if kind == 0:
+        ts = ddim_timesteps(num_inference_steps)
+        rows = []
+        for t in ts:
+            a_t, a_p = ddim_coeffs(t, num_inference_steps, ac)
+            rows.append([a_t ** 0.5, (1 - a_t) ** 0.5, a_p ** 0.5, (1 - a_p) ** 0.5, 0, 0, 0, 0])
+    else:
+        ts = dpm_timesteps(num_inference_steps)
+        rows = [list(dpmpp_2m_coeffs(i, ts, ac)) + [0, 0, 0] for i in range(num_inference_steps)]
+    return ts, rows
+
+
+def _v_solver_loop(unet, kind, num_inference_steps, guidance_scale, latents, ehs):
+    """Eager DDIM (kind 0) / DPM-Solver++(2M) (kind 1) loop of a v-prediction UNet: one fused CFG + v-step kernel per step,
+    reading its scalars from the device table through the device step counter."""
+    B, dev = latents.shape[0], latents.device
+    ts, rows = solver_table(kind, num_inference_steps)
+    coef = torch.tensor(rows, dtype=torch.float32, device=dev)
+    ctr = torch.zeros(1, device=dev, dtype=torch.int64)
+    x0_prev = torch.zeros_like(latents)
+    for t in ts:
+        x2 = torch.cat([latents, latents], 0)
+        tt = torch.full((2 * B,), float(t), device=dev)
+        v2 = unet(x2, tt, ehs).sample
+        ops.cfg_solver_step_v_dev(v2, latents, x0_prev, coef, ctr, guidance_scale, kind)
     return latents
 
 
@@ -151,13 +212,17 @@ def pndm_timesteps(num_inference_steps: int, num_train_timesteps: int = 1000, st
     return (t[:-1] + t[-2:-1] + t[-1:])[::-1]
 
 
-def pndm_rows(num_inference_steps: int, ac: List[float], num_train_timesteps: int = 1000) -> List[List[float]]:
+def pndm_rows(num_inference_steps: int, ac: List[float], num_train_timesteps: int = 1000,
+              prediction_type: str = "epsilon") -> List[List[float]]:
     """One row per model call of PNDMScheduler.step_plms, the program of cl_cfg_plms_step_dev:
     [UNet timestep, sample_coeff, eps_coeff, w_new, w_1, w_2, w_3, flags].  The update is
     x <- sample_coeff * s + eps_coeff * (w_new eps + w_1 r1 + w_2 r2 + w_3 r3), with r1..r3 the most recent pushed eps and s the
     current sample (or the sample saved at call 0, on the restart at call 1).  Call 1 re-runs the transfer of call 0
     (t + ratio -> t) from the saved sample with the mean of the two eps and does not push; every other call pushes its eps
-    and uses the Adams-Bashforth weights of the history length (at most 4)."""
+    and uses the Adams-Bashforth weights of the history length (at most 4).
+    prediction_type "v_prediction" gives the 10-column rows of cl_cfg_plms_step_v_dev: two more columns, sqrt(a) and sqrt(1 - a)
+    at the transfer's source timestep, where PNDMScheduler._get_prev_sample converts the combined v to eps."""
+    _check_prediction_type(prediction_type)
     ratio = num_train_timesteps // num_inference_steps
     rows, n_ets = [], 0
     for c, t in enumerate(pndm_timesteps(num_inference_steps, num_train_timesteps)):
@@ -179,18 +244,24 @@ def pndm_rows(num_inference_steps: int, ac: List[float], num_train_timesteps: in
         a_t = ac[t_from]
         a_p = ac[t_to] if t_to >= 0 else ac[0]
         denom = a_t * (1.0 - a_p) ** 0.5 + (a_t * (1.0 - a_t) * a_p) ** 0.5
-        rows.append([float(t), (a_p / a_t) ** 0.5, -(a_p - a_t) / denom, *(list(w) + [0.0] * (4 - len(w))), float(flags)])
+        row = [float(t), (a_p / a_t) ** 0.5, -(a_p - a_t) / denom, *(list(w) + [0.0] * (4 - len(w))), float(flags)]
+        if prediction_type == "v_prediction":
+            row += [a_t ** 0.5, (1.0 - a_t) ** 0.5]
+        rows.append(row)
     return rows
 
 
 @torch.no_grad()
 def pndm_sample(unet, control_lora, guide: Optional[torch.Tensor], cond: torch.Tensor, uncond: torch.Tensor, num_inference_steps: int = 50,
                 guidance_scale: float = 7.5, latents: Optional[torch.Tensor] = None, seed: int = 0, height: int = 512,
-                width: int = 512) -> torch.Tensor:
+                width: int = 512, prediction_type: str = "epsilon") -> torch.Tensor:
     """Same contract as ddim_sample with diffusers' PNDMScheduler (skip_prk_steps, the default scheduler of an SD-1.5
     pipeline): N + 1 UNet calls, one fused CFG + PLMS kernel per call reading its row of `pndm_rows` through a device counter."""
+    _check_prediction_type(prediction_type)
     B, dev, latents, ehs = _begin_loop(control_lora, guide, cond, uncond, latents, seed, height, width)
-    rows = torch.tensor(pndm_rows(num_inference_steps, sd15_alphas_cumprod()), dtype=torch.float32, device=dev)
+    rows = torch.tensor(pndm_rows(num_inference_steps, sd15_alphas_cumprod(), prediction_type=prediction_type), dtype=torch.float32,
+                        device=dev)
+    step = ops.cfg_plms_step_v_dev if prediction_type == "v_prediction" else ops.cfg_plms_step_dev
     ring = torch.zeros((3,) + tuple(latents.shape), device=dev, dtype=torch.float32)
     saved = torch.zeros_like(latents)
     ctr = torch.zeros(1, device=dev, dtype=torch.int64)
@@ -198,7 +269,7 @@ def pndm_sample(unet, control_lora, guide: Optional[torch.Tensor], cond: torch.T
         x2 = torch.cat([latents, latents], 0)
         tt = torch.full((2 * B,), float(t), device=dev)
         eps2 = unet(x2, tt, ehs).sample
-        ops.cfg_plms_step_dev(eps2, latents, ring, saved, rows, ctr, guidance_scale)
+        step(eps2, latents, ring, saved, rows, ctr, guidance_scale)
     return latents
 
 
@@ -217,30 +288,28 @@ class GraphedSampler:
     replays, with the eps history and the saved sample of its restart step in device buffers).
 
     control_lora = None samples without a ControlLoRA: the UNet runs with whatever processors are installed (DreamBooth LoRA
-    processors, or none for the base model), there is no hint encoder and no control product, and `guide` is None."""
+    processors, or none for the base model), there is no hint encoder and no control product, and `guide` is None.
+
+    prediction_type "v_prediction" (SD-2.1 768) reads the UNet output as v: the step kernel is the v form of the same fused
+    CFG + update (cl_cfg_solver_step_v_dev / cl_cfg_plms_step_v_dev), with the same tables (PNDM: two more columns per row)."""
 
     def __init__(self, unet, control_lora, batch: int, height: int = 512, width: int = 512, scheduler: str = "ddim",
-                 num_inference_steps: int = 50, guidance_scale: float = 7.5, scale: float = 1.0, text_dim: Optional[int] = None):
+                 num_inference_steps: int = 50, guidance_scale: float = 7.5, scale: float = 1.0, text_dim: Optional[int] = None,
+                 prediction_type: str = "epsilon"):
         if scheduler not in ("ddim", "dpmpp", "pndm"):
             raise ValueError(f"unknown scheduler {scheduler}")
+        _check_prediction_type(prediction_type)
         self.unet, self.cl = unet, control_lora
         self.B, self.h, self.w = batch, height // 8, width // 8
         self.kind = {"ddim": 0, "dpmpp": 1, "pndm": 2}[scheduler]
+        self.prediction_type = prediction_type
         self.steps, self.guidance, self.scale = int(num_inference_steps), float(guidance_scale), float(scale)
         dev = unet.device_
-        ac = sd15_alphas_cumprod()
-        if self.kind == 0:
-            ts = ddim_timesteps(self.steps)
-            rows = []
-            for t in ts:
-                a_t, a_p = ddim_coeffs(t, self.steps, ac)
-                rows.append([a_t ** 0.5, (1 - a_t) ** 0.5, a_p ** 0.5, (1 - a_p) ** 0.5, 0, 0, 0, 0])
-        elif self.kind == 1:
-            ts = dpm_timesteps(self.steps)
-            rows = [list(dpmpp_2m_coeffs(i, ts, ac)) + [0, 0, 0] for i in range(self.steps)]
-        else:
+        if self.kind == 2:
             ts = pndm_timesteps(self.steps)
-            rows = pndm_rows(self.steps, ac)
+            rows = pndm_rows(self.steps, sd15_alphas_cumprod(), prediction_type=prediction_type)
+        else:
+            ts, rows = solver_table(self.kind, self.steps)
         self.timesteps = ts
         self.calls = len(ts)                     # UNet calls per image batch: N, or N + 1 for PNDM
         self.ts_table = torch.tensor([float(t) for t in ts], dtype=torch.float32, device=dev)
@@ -265,10 +334,13 @@ class GraphedSampler:
         ops.sampler_prep(self.latents, self.x2, self.tt, self.ts_table, self.step_ctr)
         ctx = self._ctx
         pred, _, _ = self.unet.run_engine(self.x2, self.tt, self.ehs, {}, tape=None, scale=self.scale, prepared=ctx)
+        v = self.prediction_type == "v_prediction"
         if self.kind == 2:
-            ops.cfg_plms_step_dev(pred.data, self.latents, self.ring, self.saved, self.coef, self.step_ctr, self.guidance)
+            step = ops.cfg_plms_step_v_dev if v else ops.cfg_plms_step_dev
+            step(pred.data, self.latents, self.ring, self.saved, self.coef, self.step_ctr, self.guidance)
         else:
-            ops.cfg_solver_step_dev(pred.data, self.latents, self.x0_prev, self.coef, self.step_ctr, self.guidance, self.kind)
+            step = ops.cfg_solver_step_v_dev if v else ops.cfg_solver_step_dev
+            step(pred.data, self.latents, self.x0_prev, self.coef, self.step_ctr, self.guidance, self.kind)
 
     @torch.no_grad()
     def __call__(self, guide: Optional[torch.Tensor], cond: torch.Tensor, uncond: torch.Tensor, latents: Optional[torch.Tensor] = None,
@@ -350,7 +422,7 @@ class GraphedSampler:
 def generate(unet, control_lora, vae, text_encoder, guide: Optional[torch.Tensor], input_ids: torch.Tensor, uncond_input_ids: torch.Tensor,
              num_inference_steps: int = 50, guidance_scale: float = 7.5, scheduler: str = "ddim", latents: Optional[torch.Tensor] = None,
              seed: int = 0, sampler: Optional["GraphedSampler"] = None, height: int = 512, width: int = 512,
-             use_graph: bool = True) -> torch.Tensor:
+             use_graph: bool = True, prediction_type: str = "epsilon") -> torch.Tensor:
     """What the reference's validation loop and apps ask of `StableDiffusionPipeline` after `control_lora(guide)`
     (train_text_to_image_control_lora.py:824-843, apps/gradio_*2image.py:75-89, mix_lora_and_control_lora.py:153-164), on this
     package's frozen encoders: prompt / negative-prompt token ids -> text states (`text_encoder(ids)[0]`), the CFG denoise loop
@@ -360,7 +432,11 @@ def generate(unet, control_lora, vae, text_encoder, guide: Optional[torch.Tensor
     data-pipeline code).  control_lora = guide = None is the pipeline without a ControlLoRA (DreamBooth validation images with
     LoRA processors installed, train_dreambooth_lora.py:947-963; the base model's class images, :594-614); height / width then
     give the image size unless `latents` does.  use_graph = False runs a sampler's step program without capturing it.
-    Returns images [B,3,H,W] fp32 in [0,1]."""
+    prediction_type is the checkpoint scheduler's (scheduler_prediction_type); a given sampler must have been built with the
+    same one.  Returns images [B,3,H,W] fp32 in [0,1]."""
+    _check_prediction_type(prediction_type)
+    if sampler is not None and sampler.prediction_type != prediction_type:
+        raise ValueError(f"generate(prediction_type={prediction_type!r}) with a GraphedSampler built for {sampler.prediction_type!r}")
     cond = text_encoder(input_ids)[0]
     uncond = text_encoder(uncond_input_ids)[0]
     if sampler is not None:
@@ -368,7 +444,7 @@ def generate(unet, control_lora, vae, text_encoder, guide: Optional[torch.Tensor
     else:
         fn = {"ddim": ddim_sample, "dpmpp": dpmpp_sample, "pndm": pndm_sample}[scheduler]
         lat = fn(unet, control_lora, guide, cond, uncond, num_inference_steps=num_inference_steps, guidance_scale=guidance_scale,
-                 latents=latents, seed=seed, height=height, width=width)
+                 latents=latents, seed=seed, height=height, width=width, prediction_type=prediction_type)
     img = vae.decode(lat / float(vae.config.scaling_factor)).sample
     return ops.channel_affine_nchw(img.contiguous(), 0.5, torch.full((img.shape[1],), 0.5, device=img.device, dtype=torch.float32)).clamp_(0.0, 1.0)
 
@@ -377,7 +453,7 @@ def generate(unet, control_lora, vae, text_encoder, guide: Optional[torch.Tensor
 def sample_class_images(unet, vae, text_encoder, class_ids: torch.Tensor, uncond_ids: torch.Tensor, num_images: int, out_dir,
                         sample_batch_size: int = 4, num_inference_steps: int = 50, guidance_scale: float = 7.5, height: int = 512,
                         width: int = 512, seed: int = 0, sampler: Optional["GraphedSampler"] = None,
-                        use_graph: bool = True) -> List[str]:
+                        use_graph: bool = True, prediction_type: str = "epsilon") -> List[str]:
     """The prior-preservation class images of train_dreambooth_lora.py:580-620: `out_dir` is topped up to `num_images` entries
     (the entries already there are counted, only the missing images are generated), in batches of `sample_batch_size`, by the
     plain SD-1.5 pipeline - no ControlLoRA, the UNet with whatever processors are installed (none, for the base model), the
@@ -385,7 +461,8 @@ def sample_class_images(unet, vae, text_encoder, class_ids: torch.Tensor, uncond
     are converted like the pipeline's numpy_to_pil, `(x * 255).round()` to uint8, and saved through Pillow as
     `<index + existing>-<sha1 of the image bytes>.jpg`.  class_ids / uncond_ids: token ids [77] or [1, 77] of the class prompt
     and of the empty prompt (tokenisation stays with the caller).  The latents of a batch are drawn from `seed` plus the index
-    of its first new image.  Returns the paths written."""
+    of its first new image.  prediction_type is the checkpoint scheduler's ("v_prediction" for SD-2.1 768).  Returns the paths
+    written."""
     import hashlib
     from pathlib import Path
 
@@ -400,7 +477,7 @@ def sample_class_images(unet, vae, text_encoder, class_ids: torch.Tensor, uncond
     bs = int(sample_batch_size)
     if sampler is None:
         sampler = GraphedSampler(unet, None, bs, height, width, scheduler="pndm", num_inference_steps=num_inference_steps,
-                                 guidance_scale=guidance_scale)
+                                 guidance_scale=guidance_scale, prediction_type=prediction_type)
     elif sampler.cl is not None or sampler.B != bs:
         raise ValueError("sample_class_images needs a GraphedSampler without a ControlLoRA, of batch sample_batch_size")
     ids = class_ids.reshape(1, -1).expand(bs, -1).contiguous()
@@ -408,7 +485,8 @@ def sample_class_images(unet, vae, text_encoder, class_ids: torch.Tensor, uncond
     written = []
     for start in range(0, todo, bs):
         n = min(bs, todo - start)                  # the last batch runs full and keeps its first n images
-        img = generate(unet, None, vae, text_encoder, None, ids, neg, sampler=sampler, seed=seed + start, use_graph=use_graph)
+        img = generate(unet, None, vae, text_encoder, None, ids, neg, sampler=sampler, seed=seed + start, use_graph=use_graph,
+                       prediction_type=prediction_type)
         arr = (img[:n].permute(0, 2, 3, 1) * 255.0).round().to(torch.uint8).cpu().numpy()
         for i in range(n):
             image = Image.fromarray(arr[i])

@@ -33,6 +33,30 @@ SD15_CONFIG = dict(
     norm_eps=1e-5,
 )
 
+# Stable Diffusion 2.x (SD-2-base at 512², SD-2.1 at 768²; the two share the UNet).  attention_head_dim is the number of heads
+# per down block (diffusers 0.13): 5, 10, 20, 20 heads of 64 channels; proj_in / proj_out are [C, C] linears; the text states
+# are OpenCLIP-H's 1024 channels.
+SD21_CONFIG = dict(
+    SD15_CONFIG,
+    attention_head_dim=(5, 10, 20, 20),
+    cross_attention_dim=1024,
+    use_linear_projection=True,
+)
+
+
+def block_heads(cfg: dict):
+    """(down-block heads, up-block heads, mid-block heads) of `attention_head_dim`, an int or one value per block (diffusers
+    0.13: down block i takes list[i], up block i reversed(list)[i], the mid block list[-1]).  The value is the number of heads;
+    head dim = channels / heads."""
+    h = cfg["attention_head_dim"]
+    n = len(cfg["down_block_types"])
+    if isinstance(h, int):
+        return [h] * n, [h] * n, h
+    h = [int(v) for v in h]
+    if len(h) != n:
+        raise ValueError(f"attention_head_dim {tuple(h)}: one value per down block ({n}) expected")
+    return h, h[::-1], h[-1]
+
 
 class _Resnet:
     def __init__(self, sd, prefix, dev, need_dx):
@@ -81,8 +105,13 @@ class _Transformer:
 
 
 class UNetWeights:
-    """Frozen SD-1.5 UNet weights converted once to the kernels' layouts (bf16, [out, ky, kx, in], transposed copies for
-    the dX GEMMs).  `sd` uses diffusers' key names (e.g. the tensors of unet/diffusion_pytorch_model.safetensors)."""
+    """Frozen SD-1.5 / SD-2.x UNet weights converted once to the kernels' layouts (bf16, [out, ky, kx, in], transposed copies
+    for the dX GEMMs).  `sd` uses diffusers' key names (e.g. the tensors of unet/diffusion_pytorch_model.safetensors).
+
+    SD-2.x options: `attention_head_dim` per block (block_heads); `use_linear_projection` ([C, C] proj_in / proj_out weights,
+    which in channels-last layout are the same GEMM as the [C, C, 1, 1] convs, so LinearW takes either); `upcast_attention`.
+    Up-casting asks diffusers to form QK^T and the softmax in fp32; our attention kernels always compute QK^T from the bf16
+    operands with fp32 accumulation and the softmax in fp32, so the option is accepted and changes nothing here."""
 
     def __init__(self, sd: Dict[str, torch.Tensor], device, config: Optional[dict] = None):
         cfg = dict(SD15_CONFIG)
@@ -91,7 +120,7 @@ class UNetWeights:
         dev = device
         ch = list(cfg["block_out_channels"])
         layers = cfg["layers_per_block"]
-        heads = cfg["attention_head_dim"]
+        down_heads, up_heads, mid_heads = block_heads(cfg)
         self.conv_in = ConvW.make(sd["conv_in.weight"], sd["conv_in.bias"], dev, need_dx=False)
         self.time1 = LinearW.make(sd["time_embedding.linear_1.weight"], sd["time_embedding.linear_1.bias"], dev, False)
         self.time2 = LinearW.make(sd["time_embedding.linear_2.weight"], sd["time_embedding.linear_2.bias"], dev, False)
@@ -105,7 +134,7 @@ class UNetWeights:
                 blk.resnets.append(_Resnet(sd, f"down_blocks.{i}.resnets.{j}.", dev, need_dx=not first))
                 if typ == "CrossAttnDownBlock2D":
                     blk.attns.append(_Transformer(sd, f"down_blocks.{i}.attentions.{j}.", f"down_blocks.{i}.attentions.{j}.",
-                                                  dev, heads, need_dx_in=not first))
+                                                  dev, down_heads[i], need_dx_in=not first))
                 first = False
             if i != len(ch) - 1:
                 blk.down = ConvW.make(sd[f"down_blocks.{i}.downsamplers.0.conv.weight"],
@@ -118,13 +147,13 @@ class UNetWeights:
                 blk.resnets.append(_Resnet(sd, f"up_blocks.{i}.resnets.{j}.", dev, True))
                 if typ == "CrossAttnUpBlock2D":
                     blk.attns.append(_Transformer(sd, f"up_blocks.{i}.attentions.{j}.", f"up_blocks.{i}.attentions.{j}.",
-                                                  dev, heads, True))
+                                                  dev, up_heads[i], True))
             if i != len(ch) - 1:
                 blk.up = ConvW.make(sd[f"up_blocks.{i}.upsamplers.0.conv.weight"], sd[f"up_blocks.{i}.upsamplers.0.conv.bias"], dev)
             self.up.append(blk)
         self.mid = SimpleNamespace(
             resnets=[_Resnet(sd, "mid_block.resnets.0.", dev, True), _Resnet(sd, "mid_block.resnets.1.", dev, True)],
-            attn=_Transformer(sd, "mid_block.attentions.0.", "mid_block.attentions.0.", dev, heads, True))
+            attn=_Transformer(sd, "mid_block.attentions.0.", "mid_block.attentions.0.", dev, mid_heads, True))
         self.temb_cat = None
         self.norm_out = NormW.make(sd["conv_norm_out.weight"], sd["conv_norm_out.bias"], dev)
         self.conv_out_w = sd["conv_out.weight"].to(device=dev, dtype=BF16).permute(0, 2, 3, 1).contiguous()
@@ -270,8 +299,10 @@ def synthetic_state_dict(config: Optional[dict] = None, seed: int = 0) -> Dict[s
         if ci != co:
             conv(p + "conv_shortcut", co, ci, 1)
 
+    proj = (lambda name, c: lin(name, c, c)) if cfg.get("use_linear_projection", False) else (lambda name, c: conv(name, c, c, 1))
+
     def transformer(p, c):
-        norm(p + "norm", c); conv(p + "proj_in", c, c, 1)
+        norm(p + "norm", c); proj(p + "proj_in", c)
         b = p + "transformer_blocks.0."
         for n_ in ("norm1", "norm2", "norm3"):
             norm(b + n_, c)
@@ -279,7 +310,7 @@ def synthetic_state_dict(config: Optional[dict] = None, seed: int = 0) -> Dict[s
             lin(b + a + ".to_q", c, c, False); lin(b + a + ".to_k", c, kv, False); lin(b + a + ".to_v", c, kv, False)
             lin(b + a + ".to_out.0", c, c)
         lin(b + "ff.net.0.proj", 8 * c, c); lin(b + "ff.net.2", c, 4 * c)
-        conv(p + "proj_out", c, c, 1)
+        proj(p + "proj_out", c)
 
     conv("conv_in", ch[0], cfg["in_channels"], 3)
     lin("time_embedding.linear_1", temb, ch[0]); lin("time_embedding.linear_2", temb, temb)

@@ -61,6 +61,21 @@ def _control_to_var(cs: torch.Tensor, rg: bool) -> Var:
     return Var(data, rg=rg)
 
 
+def _refuse_unbuilt_options(raw: dict) -> None:
+    """config.json values that change the UNet's arithmetic and that this package does not build (the SD-2 depth, inpainting and
+    upscaler UNets, class-conditioned UNets): refused by name instead of silently ignored."""
+    def bad(key, ok):
+        if key in raw and not ok(raw[key]):
+            raise NotImplementedError(f"UNet2DConditionModel.from_pretrained: config.json {key} = {raw[key]!r} is not implemented")
+
+    bad("class_embed_type", lambda v: v is None)
+    bad("num_class_embeds", lambda v: v is None)
+    bad("only_cross_attention", lambda v: not (any(v) if isinstance(v, (list, tuple)) else v))
+    bad("dual_cross_attention", lambda v: not v)
+    bad("resnet_time_scale_shift", lambda v: v == "default")
+    bad("in_channels", lambda v: v == 4)
+
+
 class UNet2DConditionModel(nn.Module):
     def __init__(self, weights: UNetWeights):
         super().__init__()
@@ -94,9 +109,12 @@ class UNet2DConditionModel(nn.Module):
         if os.path.isfile(cfg_path):
             with open(cfg_path) as f:
                 raw = json.load(f)
+            _refuse_unbuilt_options(raw)
             keep = ("block_out_channels", "layers_per_block", "cross_attention_dim", "attention_head_dim", "in_channels",
                     "out_channels", "norm_num_groups", "norm_eps")
             config = {k: (tuple(v) if isinstance(v, list) else v) for k, v in raw.items() if k in keep}
+            # SD-2.x switches; kept only when set, so an SD-1.5 config.json loads to the same config as without them
+            config.update({k: True for k in ("use_linear_projection", "upcast_attention") if raw.get(k)})
         st = os.path.join(root, "diffusion_pytorch_model.safetensors")
         if os.path.isfile(st):
             from safetensors.torch import load_file

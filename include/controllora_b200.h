@@ -204,6 +204,9 @@ int cl_softmax_rows(const float* s, void* p, int rows, int cols, float scale, vo
  * online softmax, one CTA per (batch, head)); qkv [B*T, 3*heads*d] bf16 = q | k | v, out [B*T, heads*d] bf16. */
 int cl_clip_embed(const int64_t* ids, const void* tok, const void* pos, void* out, int rows, int T, int C, int vocab, void* stream);
 int cl_quick_gelu(void* x, int64_t n, void* stream);
+/* the exact erf GELU 0.5 x (1 + erf(x / sqrt 2)) in place on bf16 (transformers' `gelu`, CLIPMLP of SD-2's OpenCLIP-H text
+ * tower), n a positive multiple of 8 */
+int cl_gelu(void* x, int64_t n, void* stream);
 int cl_causal_attention_small(const void* qkv, void* out, int B, int T, int heads, int d, float scale, void* stream);
 int cl_channel_affine_nchw(const float* x, float* y, const float* shift, float mul, int n, int C, int64_t hw, void* stream);
 /* strided weight-space helpers of the dense (concat_hidden, models.py:208-214) control MLP: bf16 view / transpose of an fp32
@@ -231,6 +234,17 @@ int cl_cfg_solver_step_dev(const float* eps2, float* latents, float* x0_prev, co
  * step.  Reads the step from the low 32 bits of *step_ctr and advances it by 1 before the launch completes. */
 int cl_cfg_plms_step_dev(const float* eps2 /* [2B,...] = [uncond | cond] */, float* latents, float* ring, float* saved,
                          const float* rows, unsigned long long* step_ctr, int64_t n_half, float guidance, void* stream);
+/* v-prediction forms of the two device-table steps (SD-2.x 768 checkpoints: prediction_type "v_prediction").  Guidance
+ * combines the model outputs v2 = [uncond | cond] first.  cl_cfg_solver_step_v_dev takes the coef rows of
+ * cl_cfg_solver_step_dev: DDIM x0 = c0 x - c1 v, eps = c0 v + c1 x, x <- c2 x0 + c3 eps; DPM-Solver++(2M) x0 = c0 x - c1 v,
+ * then the same multistep update.  cl_cfg_plms_step_v_dev keeps the guided v in the ring and converts after the PLMS
+ * combination: rows are [num_calls][10] = the 8 columns above, then sqrt(a), sqrt(1 - a) of the transfer's source timestep,
+ * e' = sqrt(a) (w0 v + w1 r1 + w2 r2 + w3 r3) + sqrt(1 - a) s.  Both read the step from the low 32 bits of *step_ctr and
+ * advance it by 1 before the launch completes, like cl_cfg_plms_step_dev. */
+int cl_cfg_solver_step_v_dev(const float* v2, float* latents, float* x0_prev, const float* coef, unsigned long long* step_ctr,
+                             int64_t n_half, float guidance, int kind, void* stream);
+int cl_cfg_plms_step_v_dev(const float* v2 /* [2B,...] = [uncond | cond] */, float* latents, float* ring, float* saved,
+                           const float* rows, unsigned long long* step_ctr, int64_t n_half, float guidance, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * LoRA side path (diffusers LoRALinearLayer instances created at models.py:89-97,185,316-323).
