@@ -45,6 +45,12 @@ def lib() -> C.CDLL:
         _lib.cl_pose_render.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
                                         C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int,
                                         C.c_void_p, C.c_void_p, C.c_void_p]
+        _lib.cl_jpeg_scratch_bytes.restype = C.c_int64
+        _lib.cl_jpeg_scratch_bytes.argtypes = [C.c_int64, C.c_int64, C.c_int]
+        _lib.cl_jpeg_decode.restype = C.c_int
+        _lib.cl_jpeg_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int64,
+                                        C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
+                                        C.c_void_p, C.c_void_p]
         _lib.cl_cfg_plms_step_dev.restype = C.c_int
         _lib.cl_cfg_plms_step_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                               C.c_float, C.c_void_p]
@@ -189,6 +195,30 @@ class PoseLimb(C.Structure):
         ("color", C.c_int32),
         ("bx0", C.c_int32), ("by0", C.c_int32), ("bw", C.c_int32), ("bh", C.c_int32),
         ("pad_", C.c_int32),
+    ]
+
+
+class JpegImage(C.Structure):
+    """cl_jpeg_image"""
+    _fields_ = [
+        ("out_off", C.c_int64), ("coef_off", C.c_int64), ("plane_off", C.c_int64),
+        ("H", C.c_int32), ("W", C.c_int32), ("C", C.c_int32),
+        ("hmax", C.c_int32), ("vmax", C.c_int32),
+        ("mcux", C.c_int32), ("mcuy", C.c_int32), ("bpm", C.c_int32),
+        ("ri", C.c_int32), ("seg0", C.c_int32), ("nseg", C.c_int32), ("nblocks", C.c_int32),
+        ("status0", C.c_int32),
+        ("qt", C.c_int32 * 3), ("dc_tab", C.c_int32 * 3), ("ac_tab", C.c_int32 * 3),
+        ("ch", C.c_int32 * 3), ("cw", C.c_int32 * 3), ("pitch", C.c_int32 * 3), ("comp_plane", C.c_int32 * 3),
+    ]
+
+
+class JpegSegment(C.Structure):
+    """cl_jpeg_segment"""
+    _fields_ = [
+        ("data_off", C.c_int64), ("block0", C.c_int64),
+        ("nbytes", C.c_int32), ("image", C.c_int32),
+        ("mcu0", C.c_int32), ("nmcu", C.c_int32),
+        ("win0", C.c_int32), ("nwin", C.c_int32),
     ]
 
 

@@ -896,3 +896,31 @@ def pose_render(img, circles, limbs, packed: torch.Tensor, mask: torch.Tensor, o
                                     _ptr(mask), mask.numel(), out_h, out_w, int(flip), _ptr(out_canvas), _ptr(out_guide),
                                     _stream()), "cl_pose_render")
     return out_canvas, out_guide
+
+
+def jpeg_decode(p, packed: torch.Tensor, out: torch.Tensor):
+    """cl_jpeg_decode: `p` is a controllora_b200.jpeg.Packed (host descriptors, validated by the launcher, and the layout
+    of `packed`, the uint8 device buffer holding the same descriptors, the tables and the entropy-coded data: one
+    upload); `out` uint8 receives the images as packed HWC.  Synchronises once to read the per-image status.  Returns
+    (status per image as a list of ints, 0 = decoded; the rounds the window states took to reach their fixpoint)."""
+    _req(packed, torch.uint8, "packed")
+    _req(out, torch.uint8, "out")
+    if out.device != packed.device or not out.is_contiguous() or not packed.is_contiguous():
+        raise _lib.CLError(f"out: must be contiguous and on {packed.device}")
+    if packed.numel() < len(p.host):
+        raise _lib.CLError(f"packed: {packed.numel()} bytes cannot hold the {len(p.host)}-byte upload")
+    B, S = len(p.images), len(p.segments)
+    lib = _lib.lib()
+    need = lib.cl_jpeg_scratch_bytes(p.coef_blocks, p.plane_bytes, p.n_windows)
+    if need < 0:
+        check(int(need), "cl_jpeg_scratch_bytes")
+    scratch = torch.empty(need, dtype=torch.uint8, device=packed.device)
+    status = torch.empty(B + 1, dtype=torch.int32, device=packed.device)
+    base = packed.data_ptr()
+    seg_off = C.sizeof(_lib.JpegImage) * B
+    check(lib.cl_jpeg_decode(C.cast(p.images, C.c_void_p), C.c_void_p(base), B, C.cast(p.segments, C.c_void_p),
+                             C.c_void_p(base + seg_off), S, C.c_void_p(base + p.tables_off), p.tables_len,
+                             C.c_void_p(base + p.data_off), p.data_len, _ptr(scratch), need, _ptr(out), out.numel(),
+                             _ptr(status), C.c_void_p(status.data_ptr() + 4 * B), _stream()), "cl_jpeg_decode")
+    host = status.cpu().tolist()
+    return host[:B], host[B]

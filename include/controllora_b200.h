@@ -447,6 +447,66 @@ int cl_pose_render(const cl_pose_image* img, const cl_pose_image* img_dev, int B
                    int n_limbs, const uint8_t* bg, int64_t bg_bytes, uint32_t* mask, int64_t mask_words, int out_h, int out_w,
                    int flip, uint8_t* out_canvas, float* out_guide, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * K12: baseline JPEG decoder for a ragged batch, bit for bit with Pillow's libjpeg-turbo at its default settings
+ * (np.asarray(Image.open(f)) and .convert("RGB") of a YCbCr image): the image decode of train_dreambooth_lora.py:463-478
+ * (instance and class images), process/mpii_pose.py:26-27 and process/danbooru_sketch.py:33-34 (images and guides), and
+ * of the `datasets` image column of train_text_to_image_control_lora.py:615-619.
+ * Streams: sequential Huffman, 8-bit samples, one scan; 1 component (grey) or 3 (YCbCr) with luma sampling 1x1, 2x1 or
+ * 2x2 and chroma 1x1; restart intervals.  The host parses the markers and refuses everything else
+ * (controllora_b200/jpeg.py); what is decoded is restated in oracle/jpeg_ref.py.
+ *   img / img_dev: B descriptors, on the host (validated, sizes the grids) and the same bytes on the device.
+ *   seg / seg_dev: the restart segments of all images in order (one per image without restart markers), likewise; the
+ *           entropy-coded data of a segment is cut into windows of CL_JPEG_WINDOW_BITS bits, numbered consecutively
+ *           over the batch.
+ *   tables: device int32 [table_len]: quantisation tables (64 words, natural order) and Huffman tables (CL_JPEG_HUFF_WORDS
+ *           words: (length << 8 | symbol)[512] keyed by the next 9 bits, 0 for a longer code; maxcode[17]; valoff[17];
+ *           values[256]) at the offsets the descriptors name.
+ *   data:   device bytes: the segments' entropy-coded data with stuffing and markers removed, data_bytes in all.
+ *   scratch: device, scratch_bytes >= cl_jpeg_scratch_bytes(coefficient blocks, plane bytes, windows) of the batch.
+ *   out:    device uint8 [out_bytes]: image b as packed HWC (C = 1 or 3) at out_off; nothing outside those windows is
+ *           written.
+ *   status: device int32 [B]: 0, or the CL_JPEG_* bits of the corrupt entropy-coded data found (the first invalid code,
+ *           coefficient index past 63 or premature end on the sequential decoder's path).
+ *   sync_rounds: device int32 [1] or NULL: the rounds the window states took to reach their fixpoint.
+ * Seven launches whatever the data (one of them cooperative, iterating on the device), no host synchronisation.
+ * ---------------------------------------------------------------------------------------------------------- */
+enum { CL_JPEG_WINDOW_BITS = 1024, CL_JPEG_HUFF_WORDS = 810, CL_JPEG_MAX_SEGMENT_BYTES = 1 << 27 };
+enum { CL_JPEG_BAD_CODE = 1, CL_JPEG_BAD_INDEX = 2, CL_JPEG_TRUNCATED = 4, CL_JPEG_BAD_RESTART = 8 };
+
+typedef struct {
+    int64_t out_off;              /* byte offset of the image in out */
+    int64_t coef_off;             /* its first coefficient block (scan order) in the batch */
+    int64_t plane_off;            /* byte offset of its component planes in the scratch planes */
+    int32_t H, W, C;              /* size, components (1 or 3) */
+    int32_t hmax, vmax;           /* luma sampling (1 for grey) */
+    int32_t mcux, mcuy;           /* MCUs per row and column (blocks for grey) */
+    int32_t bpm;                  /* blocks per MCU */
+    int32_t ri;                   /* restart interval in MCUs, 0 = none */
+    int32_t seg0, nseg;           /* its segments */
+    int32_t nblocks;              /* mcux * mcuy * bpm */
+    int32_t status0;              /* CL_JPEG_BAD_RESTART when the host found the restart markers out of sequence */
+    int32_t qt[3], dc_tab[3], ac_tab[3];   /* table offsets in tables, per component */
+    int32_t ch[3], cw[3];         /* component sizes (libjpeg's downsampled_height / width) */
+    int32_t pitch[3];             /* plane row pitch: cw rounded up to 8 */
+    int32_t comp_plane[3];        /* byte offset of each plane from plane_off */
+} cl_jpeg_image;
+
+typedef struct {
+    int64_t data_off;             /* byte offset of its entropy-coded data in data */
+    int64_t block0;               /* its first coefficient block in the batch */
+    int32_t nbytes;               /* bytes of entropy-coded data (< CL_JPEG_MAX_SEGMENT_BYTES) */
+    int32_t image;                /* its image */
+    int32_t mcu0, nmcu;           /* its MCUs */
+    int32_t win0, nwin;           /* its windows: max(1, ceil(8 * nbytes / CL_JPEG_WINDOW_BITS)) */
+} cl_jpeg_segment;
+
+int64_t cl_jpeg_scratch_bytes(int64_t coef_blocks, int64_t plane_bytes, int n_windows);
+int cl_jpeg_decode(const cl_jpeg_image* img, const cl_jpeg_image* img_dev, int B, const cl_jpeg_segment* seg,
+                   const cl_jpeg_segment* seg_dev, int n_seg, const int32_t* tables, int64_t table_len, const uint8_t* data,
+                   int64_t data_bytes, void* scratch, int64_t scratch_bytes, uint8_t* out, int64_t out_bytes, int32_t* status,
+                   int32_t* sync_rounds, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
