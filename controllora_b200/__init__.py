@@ -12,10 +12,12 @@ from .annotator import CannyDetector, canny_batch
 from .transforms import HWC3, reference_crops, resize_image, train_transform
 from .pose import draw_bodypose, pose_batch, pose_control
 from .jpeg import decode_jpeg, dreambooth_crops, dreambooth_transform
+from .png import decode_images, decode_png
 
 __all__ = [
     "ControlLoRA", "ControlLoRAOutput", "ControlLoRACrossAttnProcessor", "ControlLoRACrossAttnProcessorV2",
     "LoRACrossAttnProcessor", "LoRALinearLayer", "UNet2DConditionModel", "AutoencoderKL", "CLIPTextModel",
     "CannyDetector", "canny_batch", "HWC3", "reference_crops", "resize_image", "train_transform",
     "draw_bodypose", "pose_batch", "pose_control", "decode_jpeg", "dreambooth_crops", "dreambooth_transform",
+    "decode_png", "decode_images",
 ]

@@ -51,6 +51,15 @@ def lib() -> C.CDLL:
         _lib.cl_jpeg_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int64,
                                         C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
                                         C.c_void_p, C.c_void_p]
+        _lib.cl_png_scratch_bytes.restype = C.c_int64
+        _lib.cl_png_scratch_bytes.argtypes = [C.c_int64, C.c_int64, C.c_int64, C.c_int]
+        _lib.cl_png_decode.restype = C.c_int
+        _lib.cl_png_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
+                                       C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p,
+                                       C.c_void_p]
+        _lib.cl_png_convert.restype = C.c_int
+        _lib.cl_png_convert.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int64,
+                                        C.c_void_p]
         _lib.cl_cfg_plms_step_dev.restype = C.c_int
         _lib.cl_cfg_plms_step_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                               C.c_float, C.c_void_p]
@@ -220,6 +229,22 @@ class JpegSegment(C.Structure):
         ("mcu0", C.c_int32), ("nmcu", C.c_int32),
         ("win0", C.c_int32), ("nwin", C.c_int32),
     ]
+
+
+class PngImage(C.Structure):
+    """cl_png_image"""
+    _fields_ = [
+        ("data_off", C.c_int64), ("raw_off", C.c_int64), ("out_off", C.c_int64),
+        ("nbytes", C.c_int32), ("H", C.c_int32), ("W", C.c_int32),
+        ("color_type", C.c_int32), ("depth", C.c_int32), ("rowbytes", C.c_int32), ("bpp", C.c_int32),
+        ("word0", C.c_int32), ("cand0", C.c_int32), ("ncand", C.c_int32), ("blk0", C.c_int32), ("nblk", C.c_int32),
+        ("pal_off", C.c_int32), ("pad_", C.c_int32),
+    ]
+
+
+class PngBlock(C.Structure):
+    """cl_png_block"""
+    _fields_ = [("out_off", C.c_int64), ("out_len", C.c_int64), ("start", C.c_int32), ("type", C.c_int32)]
 
 
 class SkinnyDesc(C.Structure):

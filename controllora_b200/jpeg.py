@@ -471,7 +471,7 @@ def pack(frames: Sequence[Frame]) -> Packed:
 
 
 # ------------------------------------------------------------------------------------------------------- public API
-def _read_source(src, i: int) -> bytes:
+def _read_source(src, i: int, what: str = "decode_jpeg") -> bytes:
     if isinstance(src, dict) and "bytes" in src:           # a datasets Image column loaded with decode=False
         src = src["bytes"] if src["bytes"] is not None else src.get("path")
     if isinstance(src, (bytes, bytearray)):
@@ -481,7 +481,7 @@ def _read_source(src, i: int) -> bytes:
     if isinstance(src, (str, os.PathLike)):
         with open(src, "rb") as fh:
             return fh.read()
-    raise CLError(f"decode_jpeg: source {i} is a {type(src).__name__}, expected bytes, bytearray, memoryview or a path")
+    raise CLError(f"{what}: source {i} is a {type(src).__name__}, expected bytes, bytearray, memoryview or a path")
 
 
 def _name(src, i: int) -> str:

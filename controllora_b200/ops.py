@@ -924,3 +924,50 @@ def jpeg_decode(p, packed: torch.Tensor, out: torch.Tensor):
                              _ptr(status), C.c_void_p(status.data_ptr() + 4 * B), _stream()), "cl_jpeg_decode")
     host = status.cpu().tolist()
     return host[:B], host[B]
+
+
+def png_decode(p, packed: torch.Tensor, out: torch.Tensor, out_channels: int, scratch: Optional[torch.Tensor] = None):
+    """cl_png_decode: `p` is a controllora_b200.png.Packed (host descriptors, validated by the launcher, and the layout of
+    `packed`, the uint8 device buffer holding the same descriptors, the palettes and the zlib streams: one upload); `out`
+    uint8 receives the images as packed HWC with out_channels = 3 (RGB) or 1 (L); `scratch`, when given, is a uint8 device
+    tensor of at least cl_png_scratch_bytes.  Synchronises once to read the per-image status and block counts.  Returns
+    (status per image as a list of ints, 0 = decoded; blocks listed per image; the device block table, int64 [slots, 3]
+    = (out_off, out_len, start | type << 32))."""
+    _req(packed, torch.uint8, "packed")
+    _req(out, torch.uint8, "out")
+    if out.device != packed.device or not out.is_contiguous() or not packed.is_contiguous():
+        raise _lib.CLError(f"out: must be contiguous and on {packed.device}")
+    if packed.numel() < len(p.host):
+        raise _lib.CLError(f"packed: {packed.numel()} bytes cannot hold the {len(p.host)}-byte upload")
+    B = len(p.images)
+    lib = _lib.lib()
+    need = lib.cl_png_scratch_bytes(p.words, p.cand_slots, p.raw_bytes, B)
+    if need < 0:
+        check(int(need), "cl_png_scratch_bytes")
+    if scratch is None:
+        scratch = torch.empty(need, dtype=torch.uint8, device=packed.device)
+    _req(scratch, torch.uint8, "scratch")
+    if scratch.device != packed.device or not scratch.is_contiguous():
+        raise _lib.CLError(f"scratch: must be contiguous and on {packed.device}")
+    blocks = torch.empty((max(p.block_slots, 1), 3), dtype=torch.int64, device=packed.device)
+    counts = torch.empty(2 * B, dtype=torch.int32, device=packed.device)
+    base = packed.data_ptr()
+    check(lib.cl_png_decode(C.cast(p.images, C.c_void_p), C.c_void_p(base), B, C.c_void_p(base + p.data_off), p.data_len,
+                            C.c_void_p(base + p.tables_off), p.tables_len, _ptr(scratch), scratch.numel(), _ptr(blocks),
+                            p.block_slots, C.c_void_p(counts.data_ptr() + 4 * B), out_channels, _ptr(out), out.numel(),
+                            _ptr(counts), _stream()), "cl_png_decode")
+    host = counts.cpu().tolist()
+    return host[:B], host[B:], blocks
+
+
+def png_convert(images, packed: torch.Tensor, src: torch.Tensor, out: torch.Tensor, out_channels: int) -> torch.Tensor:
+    """cl_png_convert: 8-bit grey or RGB rows without filter bytes in `src` (uint8, at the descriptors' raw_off) to
+    out_channels = 3 (RGB) or 1 (L) in `out`; `images` is the ctypes array of host descriptors, `packed` the same bytes on
+    the device."""
+    for name, t in (("packed", packed), ("src", src), ("out", out)):
+        _req(t, torch.uint8, name)
+        if t.device != packed.device or not t.is_contiguous():
+            raise _lib.CLError(f"{name}: must be contiguous and on {packed.device}")
+    check(_lib.lib().cl_png_convert(C.cast(images, C.c_void_p), C.c_void_p(packed.data_ptr()), len(images), _ptr(src),
+                                    src.numel(), out_channels, _ptr(out), out.numel(), _stream()), "cl_png_convert")
+    return out

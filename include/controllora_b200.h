@@ -507,6 +507,65 @@ int cl_jpeg_decode(const cl_jpeg_image* img, const cl_jpeg_image* img_dev, int B
                    int64_t data_bytes, void* scratch, int64_t scratch_bytes, uint8_t* out, int64_t out_bytes, int32_t* status,
                    int32_t* sync_rounds, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * K13: PNG decoder for a ragged batch, bit for bit with Pillow: np.asarray(Image.open(f).convert("RGB")) or
+ * .convert("L").  The PNG decode of the fill50k image and guide columns (train_text_to_image_control_lora.py:615-619,
+ * image.convert("RGB"), guide.convert("RGB")), of DiffusionDB's images in process/diffusiondb_canny.py:15-35
+ * (np.asarray(img) before cv2.Canny) and of line-art guides in process/danbooru_sketch.py:34 (.convert('L')).
+ * Every non-interlaced colour type and bit depth; the host parses the chunks and the zlib header and refuses Adam7,
+ * APNG and malformed files (controllora_b200/png.py); what is decoded is restated in oracle/png_ref.py.
+ *   img / img_dev: B descriptors, on the host (validated, sizes the grids) and the same bytes on the device.
+ *   data:   device bytes: each image's zlib stream (header, deflate data, Adler-32 trailer when present), data_bytes in all.
+ *   tables: device bytes: a 256-entry RGB palette (768 bytes, entries past PLTE black) per colour-type-3 image.
+ *   scratch: device, scratch_bytes >= cl_png_scratch_bytes(candidate words, candidate slots, inflated bytes, B).
+ *   blocks: device [n_block_slots]: the deflate blocks the stream's own chain walks through, image b's at blk0 in order;
+ *           block_count: device int32 [B], the number listed.  Empty blocks past the slots that later non-empty blocks
+ *           could need are walked but not listed.
+ *   out:    device uint8 [out_bytes]: image b as packed HWC (out_channels = 3: RGB, 1: L) at out_off; nothing outside
+ *           those windows is written.
+ *   status: device int32 [B]: 0, or CL_PNG_* bits: bad deflate data (a block type 3, bad stored lengths, an invalid
+ *           code, length code 286 / 287, distance code 30 / 31 or a distance before the stream's start), data that ends
+ *           before the last row, a filter type above 4, a wrong Adler-32.  As zlib under Pillow, decoding stops at the
+ *           first byte past the last row; the Adler-32 is compared when the stream ends exactly there with its trailer.
+ * A launch count fixed by the batch's sizes (ceil(log2(largest inflated size)) pointer-jumping rounds), no host
+ * synchronisation.
+ * cl_png_convert runs the last stage alone on 8-bit rows without filter bytes (colour type 0 or 2, rowbytes per row at
+ * raw_off in src): grey -> RGB by replication, RGB -> L by Pillow's ITU-R 601 weights (decode_images' JPEG path).
+ * ---------------------------------------------------------------------------------------------------------- */
+enum { CL_PNG_BAD_DEFLATE = 1, CL_PNG_TRUNCATED = 2, CL_PNG_BAD_FILTER = 4, CL_PNG_BAD_ADLER = 8 };
+enum { CL_PNG_MAX_SIDE = 16384, CL_PNG_MAX_STREAM_BYTES = 1 << 28 };
+
+typedef struct {
+    int64_t data_off;             /* byte offset of its zlib stream in data */
+    int64_t raw_off;              /* byte offset of its inflated rows (H x (1 + rowbytes)) in the scratch rows */
+    int64_t out_off;              /* byte offset of its pixels in out */
+    int32_t nbytes;               /* zlib stream bytes, 2 .. CL_PNG_MAX_STREAM_BYTES - 1 */
+    int32_t H, W;                 /* 1 .. CL_PNG_MAX_SIDE */
+    int32_t color_type, depth;    /* IHDR: 0 grey, 2 RGB, 3 palette, 4 grey + alpha, 6 RGBA; bits per sample */
+    int32_t rowbytes;             /* ceil(W * samples * depth / 8) */
+    int32_t bpp;                  /* filter bytes per pixel: max(1, samples * depth / 8) */
+    int32_t word0;                /* first candidate word (32 bit offsets of the stream each) in the batch: ceil(nbytes / 4) */
+    int32_t cand0, ncand;         /* its candidate slots: nbytes / 8 + 16 */
+    int32_t blk0, nblk;           /* its block-table slots: nbytes / 2 + 64 */
+    int32_t pal_off;              /* byte offset of its palette in tables (colour type 3), else 0 */
+    int32_t pad_;
+} cl_png_image;
+
+typedef struct {
+    int64_t out_off;              /* first inflated byte of the block */
+    int64_t out_len;              /* inflated bytes (as far as the stream goes) */
+    int32_t start;                /* bit offset of its header in the zlib stream */
+    int32_t type;                 /* BTYPE, | 4 when BFINAL, | 8 when the count pass decoded it (a confirmed candidate) */
+} cl_png_block;
+
+int64_t cl_png_scratch_bytes(int64_t words, int64_t cand_slots, int64_t raw_bytes, int B);
+int cl_png_decode(const cl_png_image* img, const cl_png_image* img_dev, int B, const uint8_t* data, int64_t data_bytes,
+                  const uint8_t* tables, int64_t table_bytes, void* scratch, int64_t scratch_bytes, cl_png_block* blocks,
+                  int64_t n_block_slots, int32_t* block_count, int out_channels, uint8_t* out, int64_t out_bytes,
+                  int32_t* status, void* stream);
+int cl_png_convert(const cl_png_image* img, const cl_png_image* img_dev, int B, const uint8_t* src, int64_t src_bytes,
+                   int out_channels, uint8_t* out, int64_t out_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
